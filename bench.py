@@ -2,7 +2,7 @@
 """bench.py — consensus reads/sec of the UMI-consensus hot path (BASELINE.json metric).
 
 N=1 workload = BASELINE.json configs[1]: simplex consensus, 10 M families, depth 8, 150 bp,
-substitution error rate 1e-3, synthetic (generator: fgumi_b200/synth.py), one B200.
+substitution error rate 1e-3, synthetic (generator: fgumi_b200/synth.py), one H100.
 A "step" = one pass of the hot path (ONE kernel launch through fgb_vote_device) over the whole
 batch, inputs resident in HBM.  N>1: every rank owns its own 10 M-family shard (families shard
 trivially; weak scaling), no data-path collective; the end-of-run device counters are summed with
@@ -57,17 +57,7 @@ def measured_peak_gbs():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def recorded_traffic():
-    """dram bytes per launch of vote_kernel from the committed ncu --set full capture, if any."""
-    p = os.path.join(ROOT, "profiles", "vote_kernel_traffic.json")
-    try:
-        with open(p) as f:
-            return json.load(f)
-    except Exception:
-        return None
+        return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 def cpu_quota() -> int:
@@ -389,6 +379,26 @@ def _sum_ranks(torch, dist, dev, world, r):
     return r
 
 
+DUMP_FAMILIES = 16384       # 16 k families x 150 positions x 4 columns x 4 bytes = 39 MB
+
+
+def dump_outputs(path, torch, out, host):
+    """What the last timed step handed its caller -- the four consensus columns -- for a fixed, seeded sample of
+    families (every called position of each), as float32 [families, READ_LEN] arrays, plus the sampled family
+    indices.  The timed batch is generated from fixed seeds, so two builds can be compared output for output."""
+    n = min(DUMP_FAMILIES, host.n_units)
+    fam = np.sort(np.random.default_rng(2024).choice(host.n_units, size=n, replace=False))
+    offs = host.units["out_off"][fam].astype(np.int64)
+    idx = torch.from_numpy(offs).to(out.base.device)[:, None] + torch.arange(READ_LEN, device=out.base.device)[None, :]
+    os.makedirs(path, exist_ok=True)
+    for name, col in (("base", out.base), ("qual", out.qual), ("depth", out.depth), ("errors", out.errors)):
+        a = col[idx].cpu().numpy()
+        if a.dtype == np.int16:
+            a = a.view(np.uint16)
+        np.save(os.path.join(path, f"{name}.npy"), a.astype(np.float32))
+    np.save(os.path.join(path, "family_index.npy"), fam.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -402,7 +412,11 @@ def main():
     ap.add_argument("--record-families", type=int, default=int(os.environ.get("FGB_RECORD_FAMILIES", "200000")),
                     help="families per batch of the record-level leg")
     ap.add_argument("--no-modes", action="store_true", help="skip the duplex / CODEC / Zipf kernel legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a fixed sample of the last timed step's consensus columns to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.warmup < 3:
         args.warmup = 3
 
@@ -492,14 +506,13 @@ def main():
     k_ms = float(np.mean(per_launch_ms))
     achieved = abytes / (k_ms * 1e-3) / 1e9
     peak, peak_src = measured_peak_gbs()
-    tr = recorded_traffic()
-    traffic = None
-    if tr and tr.get("units") and tr.get("dram_bytes_per_launch"):
-        traffic = tr["dram_bytes_per_launch"] * (h.n_units / tr["units"])
     roofline = {"bound": "hbm", "kernel": "vote_kernel", "achieved": achieved, "peak": peak,
-                "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+                "unit": "GB/s", "frac": achieved / peak,
                 "algorithmic_bytes_per_launch": abytes, "bytes_per_unit": abytes / h.n_units,
                 "kernel_ms": k_ms, "peak_source": peak_src}
+
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, torch, out, tb.host)
 
     # ---- e2e: host-buffer call, pinned host memory, H2D + vote + D2H inside the timed region ----
     e2e = None

@@ -1,6 +1,6 @@
-"""fgumi_b200 — Blackwell-native UMI consensus engine (drop-in for fgumi's consensus hot path).
+"""fgumi_b200 — Hopper-native UMI consensus engine (drop-in for fgumi's consensus hot path).
 
-The product is libfgumi_b200.so (hand-written sm_100a CUDA behind the C-ABI in
+The product is libfgumi_b200.so (hand-written sm_90a CUDA behind the C-ABI in
 include/fgumi_b200.h).  This package is the thin host-side mirror of that boundary.
 """
 from .engine import (Engine, PackedBatch, HostColumns, DeviceBatch, DeviceColumns,  # noqa: F401

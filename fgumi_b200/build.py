@@ -1,4 +1,4 @@
-"""In-tree build of libfgumi_b200.so with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""In-tree build of libfgumi_b200.so with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -10,11 +10,11 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libfgumi_b200.so")
 SOURCES = ["capi.cu", "host_tables.cpp", "host/caller_host.cpp", "host/bgzf.cpp"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-maxrregcount=112",      # upper bound only; vote_kernel must land at <= 96 (see _check_vote_kernel)
     "-fmad=false",            # no FMA contraction anywhere near the f64 vote (DESIGN.md numerics)
     "-Xcompiler", "-fPIC", "-shared",
-    # host code (record parsing / assembly loops): AVX2-class auto-vectorisation; every B200 host has it
+    # host code (record parsing / assembly loops): AVX2-class auto-vectorisation; every H100 host has it
     "-Xcompiler", "-march=x86-64-v3", "-Xcompiler", "-ffp-contract=off",
 ]
 

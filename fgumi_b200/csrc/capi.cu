@@ -218,7 +218,7 @@ const char* fgb_strerror(fgb_status s) {
     case FGB_OK: return "ok";
     case FGB_ERR_INVALID_ARG: return "invalid argument";
     case FGB_ERR_CUDA: return "CUDA runtime error";
-    case FGB_ERR_NO_DEVICE: return "no usable sm_100 CUDA device (this engine has no CPU fallback)";
+    case FGB_ERR_NO_DEVICE: return "no usable sm_90 CUDA device (this engine has no CPU fallback)";
     case FGB_ERR_LAYOUT: return "batch violates the SoA layout rules";
     case FGB_ERR_UNIT_TOO_LARGE: return "unit exceeds the supported size";
     case FGB_ERR_NOMEM: return "out of memory";
@@ -252,7 +252,7 @@ fgb_status fgb_create(int device, const fgb_params* params, fgb_handle** out) {
   }
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return FGB_ERR_NO_DEVICE;
-  if (prop.major != 10) return FGB_ERR_NO_DEVICE;   // kernels are sm_100a only
+  if (prop.major != 9 || prop.minor != 0) return FGB_ERR_NO_DEVICE;   // kernels are sm_90a only
   fgb_handle* h = new (std::nothrow) fgb_handle();
   if (!h) return FGB_ERR_NOMEM;
   h->device = device;

@@ -1,6 +1,6 @@
-// K2 (duplex) and K3 (CODEC) strand-combine kernels for sm_100a — pure integer/byte work.
+// K2 (duplex) and K3 (CODEC) strand-combine kernels for sm_90a — pure integer/byte work.
 //
-// Replaces (reference = /root/reference/crates/fgumi-consensus/src/):
+// Replaces (reference = fgumi 0.2.0, crates/fgumi-consensus/src/):
 //   duplex_caller.rs:838-1015   DuplexConsensusCaller::duplex_consensus (methylation disabled)
 //   codec_caller.rs:507-520     reverse_complement_ss
 //   codec_caller.rs:980-1023    pad_consensus (lowercase 'n', Q0, depth 0, errors 0)
@@ -321,7 +321,7 @@ __global__ void __launch_bounds__(kCombineThreads) duplex_combine_kernel(const D
 // settles each job's arm (:852-882) in shared memory; pass 2 combines the both-strand jobs (:912-951); the rare
 // single-strand arms and the layouts the word path does not take are redone by duplex_job_warp.
 #ifndef FGB_DUPLEX_CHUNK
-#define FGB_DUPLEX_CHUNK 256   // measured on B200 (10 M jobs): 32 -> 7.94 ms, 64 -> 6.99, 128 -> 6.76, 256 -> 6.58
+#define FGB_DUPLEX_CHUNK 256
 #endif
 constexpr int kDuplexDescCache = 8;          // row descriptors of a job kept in shared memory (4 + 4 reads per strand fit)
 constexpr int kDuplexChunk = FGB_DUPLEX_CHUNK;     // 32, 64, 128 or 256: jobs whose descriptors are fetched in one round
@@ -683,7 +683,7 @@ __global__ void __launch_bounds__(kCombineThreads) codec_combine_kernel(const Co
 // (depths, errors).  Complementing both strands at once commutes with every comparison the rule makes as long as
 // all bases are A/C/G/T/N or the pad 'n'; a job with any other byte is redone by codec_job_scalar.
 #ifndef FGB_CODEC_CHUNK
-#define FGB_CODEC_CHUNK 256    // B200, 2 M jobs: 32 -> 2.62 ms, 128 / 256 -> 2.55 (issue-bound either way)
+#define FGB_CODEC_CHUNK 256
 #endif
 constexpr int kCodecChunk = FGB_CODEC_CHUNK;     // 32 .. 256 (power of two): units / jobs whose descriptors are fetched in one round
 

@@ -1,7 +1,7 @@
 // f64 log-space helpers evaluated on the device for positions that leave the integer fast path.
 //
-// Behavioural spec: /root/reference/crates/fgumi-consensus/src/phred.rs (cited per function).
-// Add/sub/mul/div are IEEE-754 correctly rounded on sm_100a exactly as on the host, so the Kahan
+// Behavioural spec: fgumi 0.2.0, crates/fgumi-consensus/src/phred.rs (cited per function).
+// Add/sub/mul/div are IEEE-754 correctly rounded on sm_90a exactly as on the host, so the Kahan
 // likelihood sums, the tie test and the threshold compares are bit-identical to the reference's.
 // exp/log/log1p/expm1 come from CUDA's libdevice (<= 1-2 ulp) rather than glibc; their results only
 // reach the output through floor(x + 0.001), so a difference needs x within ~1e-15 of an integer

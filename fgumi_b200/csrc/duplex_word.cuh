@@ -1,7 +1,7 @@
 // The duplex strand combine on one 8-position word, shared by the standalone word kernel (combine_kernels.cuh) and the
 // vote kernels' duplex epilogue (vote_kernel.cuh).  Pure byte-parallel integer work.
 //
-// Replaces (reference = /root/reference/crates/fgumi-consensus/src/duplex_caller.rs):
+// Replaces (reference = fgumi 0.2.0, crates/fgumi-consensus/src/duplex_caller.rs):
 //   :912-927  agreement / disagreement rule (sum capped at 93; higher quality wins with the difference; equal -> Q2)
 //   :930-935  N propagation and the Q2 mask
 //   :943-951  exact error recount against the pooled source reads (is_error, :797-800)

@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(256) filter_simplex_kernel(const FilterArgs a)
 // folded inside the warp first (items of one unit sit on consecutive lanes: a segmented shuffle reduction) and then
 // into shared memory by the first lane of each run.
 #ifndef FGB_FILTER_CHUNK
-#define FGB_FILTER_CHUNK 256   // B200, 4 M units: 32 -> 1.68 ms, 128 -> 1.35, 256 -> 1.30
+#define FGB_FILTER_CHUNK 256
 #endif
 constexpr int kFilterChunk = FGB_FILTER_CHUNK;     // 32 .. 256 (power of two): units / jobs whose descriptors are fetched in one round
 

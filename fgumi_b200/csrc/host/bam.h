@@ -1,6 +1,6 @@
 // Host-side BAM record access and consensus-record assembly (product code, header-only).
 //
-// Behavioural spec (reference = /root/reference/crates/):
+// Behavioural spec (reference = fgumi 0.2.0, crates/):
 //   fgumi-raw-bam/src/fields.rs:6-23,240-265,289-310,393-502   record layout, flags, aux walking
 //   fgumi-raw-bam/src/sequence.rs:9-35,148-209                 4-bit sequence codec
 //   fgumi-raw-bam/src/cigar.rs:50-70,82-101,137-150,294-306,514-573   CIGAR helpers, MC parsing

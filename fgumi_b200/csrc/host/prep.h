@@ -1,7 +1,7 @@
 // Shared host-side preparation code of the record-level callers (product code, header-only):
 // source-read creation, CIGAR grouping, RX consensus and the SoA batch packer.
 //
-// Behavioural spec (reference = /root/reference/crates/fgumi-consensus/src/):
+// Behavioural spec (reference = fgumi 0.2.0, crates/fgumi-consensus/src/):
 //   vanilla_caller.rs:47-119    select_most_common_alignment_group
 //   vanilla_caller.rs:780-804   find_quality_trim_point
 //   vanilla_caller.rs:863-955   create_source_read

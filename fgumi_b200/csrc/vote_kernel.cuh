@@ -1,6 +1,6 @@
-// K1 — simplex / single-strand consensus vote for sm_100a.
+// K1 — simplex / single-strand consensus vote for sm_90a.
 //
-// Replaces (reference = /root/reference/crates/fgumi-consensus/src/):
+// Replaces (reference = fgumi 0.2.0, crates/fgumi-consensus/src/):
 //   vanilla_caller.rs:1260-1358  create_consensus_from_source_reads (position loop, thresholds,
 //                                single-read LUT path)
 //   base_builder.rs:295-327      ConsensusBaseBuilder::add   (4-lane f64 Kahan likelihoods)
@@ -1992,10 +1992,12 @@ __device__ __forceinline__ void vote_kernel_body(const Args& a) {
 
 // Three instantiations, one per tile class (fgb_config.h): the planner cuts class-homogeneous tiles and the
 // engine launches each kernel on its own run of the (class-sorted) tile array.  Every one of them is correct
-// for any tile; they differ in how the work of a tile is dealt to the threads.
-__global__ void __launch_bounds__(kThreads) vote_kernel(const VoteArgs a) { vote_kernel_body<0>(a); }
-__global__ void __launch_bounds__(kThreads) vote_kernel_shallow(const VoteArgs a) { vote_kernel_body<1>(a); }
-__global__ void __launch_bounds__(kThreads) vote_kernel_deep(const VoteArgs a) { vote_kernel_body<2>(a); }
+// for any tile; they differ in how the work of a tile is dealt to the threads.  Two CTAs per SM is the design point
+// (DESIGN.md section 3); without the minimum-blocks bound ptxas for sm_90a caps them at 72 registers and spills in
+// the item loop.
+__global__ void __launch_bounds__(kThreads, 2) vote_kernel(const VoteArgs a) { vote_kernel_body<0>(a); }
+__global__ void __launch_bounds__(kThreads, 2) vote_kernel_shallow(const VoteArgs a) { vote_kernel_body<1>(a); }
+__global__ void __launch_bounds__(kThreads, 2) vote_kernel_deep(const VoteArgs a) { vote_kernel_body<2>(a); }
 // The same three with the duplex epilogue (fgb_vote_duplex_device).
 __global__ void __launch_bounds__(kThreads, 2) vote_kernel_duplex(const VoteArgsDuplex a) { vote_kernel_body<0, true, VoteArgsDuplex>(a); }
 __global__ void __launch_bounds__(kThreads, 2) vote_kernel_shallow_duplex(const VoteArgsDuplex a) { vote_kernel_body<1, true, VoteArgsDuplex>(a); }

@@ -238,7 +238,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  fgumi_b200 has no CPU fallback.")
+            "(nvcc, sm_90a).  fgumi_b200 has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     vp, u64, u32 = C.c_void_p, C.c_uint64, C.c_uint32
     lib.fgb_abi_version.restype = u32

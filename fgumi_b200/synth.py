@@ -1,6 +1,6 @@
 """Synthetic grouped-family generator (restates the model of `fgumi simulate grouped-reads`).
 
-Model (reference, /root/reference/src/lib/):
+Model (reference, fgumi 0.2.0 src/lib/):
   * template bases uniform over ACGT; every read of a family copies the template
     (commands/simulate/grouped_reads.rs:530-556);
   * qualities from PositionQualityModel::default — ramp 25->37 over the first 10 bases, 37 flat,

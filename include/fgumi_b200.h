@@ -1,5 +1,5 @@
 /*
- * fgumi_b200.h — C-ABI of the B200-native UMI-consensus engine.
+ * fgumi_b200.h — C-ABI of the H100-native UMI-consensus engine.
  *
  * This is the drop-in boundary for fgumi's consensus hot path.  The reference (fgumi 0.2.0,
  * pure Rust, `#![deny(unsafe_code)]`) has no FFI; its only boundary is the trait
@@ -57,7 +57,7 @@ enum {
   FGB_OK = 0,
   FGB_ERR_INVALID_ARG = 1,   /* null pointer, bad size, bad params                           */
   FGB_ERR_CUDA = 2,          /* a CUDA runtime call failed; see fgb_last_error()              */
-  FGB_ERR_NO_DEVICE = 3,     /* no usable sm_100 device — the engine has NO CPU fallback      */
+  FGB_ERR_NO_DEVICE = 3,     /* no usable sm_90 device — the engine has NO CPU fallback       */
   FGB_ERR_LAYOUT = 4,        /* batch violates the layout rules above (alignment, ranges)     */
   FGB_ERR_UNIT_TOO_LARGE = 5,/* a single unit exceeds fgb_tile_capacity_bytes()               */
   FGB_ERR_NOMEM = 6,

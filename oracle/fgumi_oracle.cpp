@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE — NOT PRODUCT CODE.  See fgumi_oracle.hpp for the rules.
 // CPU restatement of fgumi-consensus {phred,base_builder,vanilla_caller,duplex_caller,
-// codec_caller}.rs hot loops.  Citations are relative to /root/reference/crates/fgumi-consensus/src/.
+// codec_caller}.rs hot loops.  Citations are relative to fgumi 0.2.0's crates/fgumi-consensus/src/.
 #include "fgumi_oracle.hpp"
 
 #include <algorithm>

@@ -13,7 +13,7 @@
 // reproduced in tests/test_oracle_kat.py.  Record-level byte parity against the Rust binary is
 // "parity unpinned" (the reference has no golden outputs and cannot be run here); see DESIGN.md.
 //
-// All `file:line` citations are relative to /root/reference/.
+// All `file:line` citations are relative to the fgumi 0.2.0 source tree.
 #pragma once
 #include <cstddef>
 #include <cstdint>

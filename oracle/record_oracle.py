@@ -3,7 +3,7 @@
 Record-level restatement (pure Python, small cases only) of the HOST side of fgumi's consensus
 callers: raw BAM record decoding, source-read preparation, CIGAR grouping, the group / orphan rules
 and consensus-record assembly.  The per-position vote itself is delegated to the C++ oracle
-(oracle/liboracle.so).  Only tests/ may import this.  Citations are relative to /root/reference/.
+(oracle/liboracle.so).  Only tests/ may import this.  Citations are relative to the fgumi 0.2.0 source tree.
 
 Parity status: the reference has no golden outputs and cannot be built here, so byte-level parity
 with the fgumi binary is "parity unpinned"; this file is checked against the reference's own

@@ -7,6 +7,7 @@ import gzip
 import os
 import struct
 import sys
+import tempfile
 import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -73,7 +74,7 @@ def read_bam_records(path):
 
 def main():
     G = int(sys.argv[1]) if len(sys.argv) > 1 else 3000
-    out_dir = sys.argv[2] if len(sys.argv) > 2 else "gpurun_out"
+    out_dir = sys.argv[2] if len(sys.argv) > 2 else os.path.join(tempfile.gettempdir(), "fgumi_file_level")
     os.makedirs(out_dir, exist_ok=True)
     rng = np.random.default_rng(99)
     t0 = time.perf_counter()

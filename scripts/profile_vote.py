@@ -1,5 +1,5 @@
-"""Profiling driver (GPU box): build one synthetic batch in HBM and launch the vote kernel a few
-times — meant to be wrapped by ncu (see profiles/README.md)."""
+"""Profiling driver: build one synthetic batch in device memory and launch the vote kernel a few
+times, timed with CUDA events (usage: python scripts/profile_vote.py [units] [depth|zipf] [launches])."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import ctypes as C

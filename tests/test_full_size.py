@@ -1,11 +1,11 @@
-"""BASELINE.json's configurations at FULL size on one B200, checked through size-independent
+"""BASELINE.json's configurations at FULL size on one H100 (80 GB), checked through size-independent
 properties plus an exact oracle comparison on a random sample of families (the oracle cannot vote
 10 M families in seconds, but it can vote a few thousand of them drawn from the very same batch):
 
   cfg 2  simplex  10 M families, depth 8, 150 bp, error 1e-3
   cfg 3  duplex   5 M molecules, 4+4 reads per strand  (20 M single-strand units -> 10 M duplex reads)
   cfg 4  CODEC    2 M molecules, depth 2-20 per strand, 2 x 150 bp
-  cfg 5  simplex  12.5 M families (one rank's shard of 100 M), Zipf depth 1-100
+  cfg 5  simplex  6.25 M families (one rank's shard of 100 M over 16 GPUs), Zipf depth 1-100
 
 Besides the sample, one contiguous slice of every vote (up to 2 M source rows: 250 k families at depth 8) is
 compared with a full oracle pass, every unit and position.
@@ -175,7 +175,7 @@ def test_config2_simplex_10m_depth8(fg):
 def test_config5_zipf_shard(fg):
     import torch
     from fgumi_b200 import synth
-    U = max(1000, int(12_500_000 * SCALE))
+    U = max(1000, int(6_250_000 * SCALE))          # ~120 M source rows (37 GB) + two output sets
     depths = synth.zipf_depths(U, 1, 100, 1.0, seed=42 + 3)          # rank 3's shard: seed 42+rank
     tb = synth.device_batch(torch, DEV, depths, L, 1e-3, seed=45)
     eng, out = _vote_and_check(fg, torch, tb, depths, n_sample=600, seed=5)

@@ -143,3 +143,40 @@ def test_clock_sampler_uses_the_samples_inside_the_timed_region():
     c = b.ClockSampler(0, [sys.executable, "-c", "print('garbage')"])
     c.start(); c.begin(); c.end()
     assert c.stop()["sm_mhz"] is None
+
+
+def test_bench_dump_outputs_writes_a_fixed_float_sample(tmp_path):
+    """`bench.py --dump-outputs DIR`: the four consensus columns of a fixed, seeded sample of families, every called
+    position of each, as float32 .npy (plus the sampled family indices), well under 64 MB."""
+    import importlib.util
+    from types import SimpleNamespace
+    import torch
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    spec = importlib.util.spec_from_file_location("bench_mod", os.path.join(root, "bench.py"))
+    b = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(b)
+    U, Lo = 20000, 152
+    units = np.zeros(U + 1, dtype=[("out_off", "<u8"), ("read_begin", "<u4"), ("cons_len", "<u4")])
+    units["out_off"] = np.arange(U + 1, dtype=np.uint64) * np.uint64(Lo)
+    host = SimpleNamespace(n_units=U, units=units)
+    g = torch.Generator().manual_seed(1)
+    out = SimpleNamespace(base=torch.randint(0, 256, (U * Lo,), dtype=torch.uint8, generator=g),
+                          qual=torch.randint(0, 94, (U * Lo,), dtype=torch.uint8, generator=g),
+                          depth=torch.randint(0, 40000, (U * Lo,), generator=g).to(torch.int16),
+                          errors=torch.randint(0, 9, (U * Lo,), generator=g).to(torch.int16))
+    b.dump_outputs(str(tmp_path / "a"), torch, out, host)
+    b.dump_outputs(str(tmp_path / "b"), torch, out, host)
+    names = ("base", "qual", "depth", "errors", "family_index")
+    total = 0
+    fam = np.load(tmp_path / "a" / "family_index.npy").astype(np.int64)
+    assert len(fam) == b.DUMP_FAMILIES and np.all(np.diff(fam) > 0)
+    for name in names:
+        x, y = np.load(tmp_path / "a" / f"{name}.npy"), np.load(tmp_path / "b" / f"{name}.npy")
+        assert x.dtype in (np.float32, np.float64) and np.array_equal(x, y)
+        total += x.nbytes
+        if name != "family_index":
+            col = getattr(out, name).numpy()
+            col = col.view(np.uint16) if col.dtype == np.int16 else col
+            want = col.reshape(U, Lo)[fam, :b.READ_LEN]
+            assert x.shape == want.shape and np.array_equal(x, want.astype(np.float32))
+    assert total <= 64 << 20

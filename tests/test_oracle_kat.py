@@ -1,6 +1,6 @@
 """Pins the CPU oracle against every known-answer test the reference holds for the hot path
 (SURVEY.md §8c).  Each test names the reference test it reproduces
-(/root/reference/crates/fgumi-consensus/src/<file>:<line>).  CPU only.
+(fgumi 0.2.0: crates/fgumi-consensus/src/<file>:<line>).  CPU only.
 """
 import ctypes as C
 import math

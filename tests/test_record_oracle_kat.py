@@ -1,6 +1,6 @@
 """Pins the Python record-level oracle (oracle/record_oracle.py) against the reference's own
 known-answer unit tests for the host side of the simplex caller.  Each test names the reference test
-it reproduces (/root/reference/crates/...).  CPU only."""
+it reproduces (fgumi 0.2.0: crates/...).  CPU only."""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a vote (through the C-ABI) against the CPU oracle on identical inputs.
+"""GPU parity: the sm_90a vote (through the C-ABI) against the CPU oracle on identical inputs.
 
 Bar (BASELINE.json north_star): consensus bases, depths, errors and lengths bit-exact; consensus
 qualities within +-1 phred (the tests additionally report how many differ at all — expected 0)."""
