@@ -105,7 +105,6 @@ struct fgb_handle {
   struct TraceMark { cudaEvent_t ev; const char* what; int chunk; };
   std::vector<TraceMark> trace_ev;                  // device timeline of the last submit
   std::chrono::steady_clock::time_point trace_t0, trace_t1;
-  int vote_variant = 1;                             // FGB_VOTE_KERNEL=0: the general kernel votes every tile (A/B runs)
   uint8_t* d_dstatus = nullptr; uint64_t cap_dstatus = 0;   // fgb_vote_duplex_device: job status bytes when the caller wants none
 };
 
@@ -161,7 +160,7 @@ fgb_status launch_vote(fgb_handle* h, const fgb_batch& b, const fgb_columns& out
   }
   const uint64_t max_grid = static_cast<uint64_t>(h->sm_count) * 2u;
   const uint64_t c0 = b.class_tiles[0], c1 = b.class_tiles[1], c2 = b.class_tiles[2];
-  const bool sorted = h->vote_variant != 0 && c0 + c1 + c2 == b.n_tiles;
+  const bool sorted = c0 + c1 + c2 == b.n_tiles;
   auto launch = [&](int cls, uint64_t first, uint64_t n) {
     if (!n) return;
     VoteArgsDuplex x = a;
@@ -261,7 +260,6 @@ fgb_status fgb_create(int device, const fgb_params* params, fgb_handle** out) {
   if (const char* e = std::getenv("FGB_SUBMIT_CHUNK_MB"))
     { h->chunk_bytes = static_cast<uint64_t>(std::max(1, std::atoi(e))) << 20; h->chunk_bytes_set = true; }
   if (const char* e = std::getenv("FGB_SUBMIT_TRACE")) h->trace = std::atoi(e) != 0;
-  if (const char* e = std::getenv("FGB_VOTE_KERNEL")) h->vote_variant = std::atoi(e) ? 1 : 0;
   h->params = *params;
   build_host_tables(params->error_rate_pre_umi, params->error_rate_post_umi, &h->host_tables);
 
@@ -1293,137 +1291,6 @@ fgb_status fgb_codec_combine_device(fgb_handle* h, const fgb_batch* in, const fg
   }
   h->launches++;
   FGB_CUDA(h, cudaGetLastError());
-  return FGB_OK;
-}
-
-}  // extern "C"
-
-// ---- host-buffer vote + combine -------------------------------------------------------------------
-namespace {
-
-// RAII bundle of device allocations for the one-shot submit calls.
-struct DevPool {
-  std::vector<void*> ptrs;
-  ~DevPool() { for (void* p : ptrs) cudaFree(p); }
-  template <class T> cudaError_t alloc(T** p, uint64_t n) {
-    cudaError_t e = cudaMalloc(reinterpret_cast<void**>(p), (n ? n : 1) * sizeof(T) + 64);
-    if (e == cudaSuccess) ptrs.push_back(*p);
-    return e;
-  }
-};
-
-struct DeviceBatchCopy {
-  fgb_batch b{};
-  fgb_columns ss{};
-};
-
-// Copies a whole host batch to fresh device buffers and votes it on `s`.
-fgb_status upload_and_vote(fgb_handle* h, const fgb_batch* in, DevPool* pool, DeviceBatchCopy* d,
-                           cudaStream_t s) {
-  uint8_t *bases = nullptr, *quals = nullptr;
-  uint64_t* reads = nullptr;
-  fgb_unit* units = nullptr;
-  fgb_tile* tiles = nullptr;
-  const uint64_t nb = (in->n_bytes + 15u) & ~15ull;
-  FGB_CUDA(h, pool->alloc(&bases, nb + 16));
-  FGB_CUDA(h, pool->alloc(&quals, nb + 16));
-  FGB_CUDA(h, pool->alloc(&reads, in->n_reads + 2));
-  FGB_CUDA(h, pool->alloc(&units, in->n_units + 1));
-  FGB_CUDA(h, pool->alloc(&tiles, in->n_tiles));
-  FGB_CUDA(h, pool->alloc(&d->ss.base, in->n_out + 8));
-  FGB_CUDA(h, pool->alloc(&d->ss.qual, in->n_out + 8));
-  FGB_CUDA(h, pool->alloc(&d->ss.depth, in->n_out + 8));
-  FGB_CUDA(h, pool->alloc(&d->ss.errors, in->n_out + 8));
-  FGB_CUDA(h, cudaMemcpyAsync(bases, in->bases, in->n_bytes, cudaMemcpyHostToDevice, s));
-  FGB_CUDA(h, cudaMemcpyAsync(quals, in->quals, in->n_bytes, cudaMemcpyHostToDevice, s));
-  FGB_CUDA(h, cudaMemcpyAsync(reads, in->reads, in->n_reads * 8, cudaMemcpyHostToDevice, s));
-  FGB_CUDA(h, cudaMemcpyAsync(units, in->units, (in->n_units + 1) * sizeof(fgb_unit), cudaMemcpyHostToDevice, s));
-  FGB_CUDA(h, cudaMemcpyAsync(tiles, in->tiles, in->n_tiles * sizeof(fgb_tile), cudaMemcpyHostToDevice, s));
-  d->b = *in;
-  d->b.class_tiles[0] = d->b.class_tiles[1] = d->b.class_tiles[2] = 0;   // tiles uploaded as planned: general kernel
-  d->b.bases = bases; d->b.quals = quals; d->b.reads = reads; d->b.units = units; d->b.tiles = tiles;
-  return launch_vote(h, d->b, d->ss, s);
-}
-
-fgb_status download_ss(fgb_handle* h, const DeviceBatchCopy& d, const fgb_columns* ss_out, uint64_t n,
-                       cudaStream_t s) {
-  if (!ss_out || !n) return FGB_OK;
-  FGB_CUDA(h, cudaMemcpyAsync(ss_out->base, d.ss.base, n, cudaMemcpyDeviceToHost, s));
-  FGB_CUDA(h, cudaMemcpyAsync(ss_out->qual, d.ss.qual, n, cudaMemcpyDeviceToHost, s));
-  FGB_CUDA(h, cudaMemcpyAsync(ss_out->depth, d.ss.depth, n * 2, cudaMemcpyDeviceToHost, s));
-  FGB_CUDA(h, cudaMemcpyAsync(ss_out->errors, d.ss.errors, n * 2, cudaMemcpyDeviceToHost, s));
-  return FGB_OK;
-}
-
-}  // namespace
-
-extern "C" {
-
-fgb_status fgb_duplex_submit(fgb_handle* h, const fgb_batch* in, const fgb_columns* ss_out,
-                             const fgb_duplex_job* jobs, uint64_t n_jobs, uint64_t n_duplex_out,
-                             const fgb_duplex_out* out) {
-  if (!h || !in || !ss_out || (n_jobs && (!jobs || !out))) return FGB_ERR_INVALID_ARG;
-  if (in->n_tiles == 0) return FGB_OK;
-  FGB_CUDA(h, cudaSetDevice(h->device));
-  cudaStream_t s = h->slots[0].stream;
-  DevPool pool;
-  DeviceBatchCopy d;
-  fgb_status st = upload_and_vote(h, in, &pool, &d, s);
-  if (st != FGB_OK) return st;
-  if ((st = download_ss(h, d, ss_out, in->n_out, s)) != FGB_OK) return st;
-  if (n_jobs) {
-    fgb_duplex_job* djobs = nullptr;
-    fgb_duplex_out dout{};
-    FGB_CUDA(h, pool.alloc(&djobs, n_jobs));
-    FGB_CUDA(h, pool.alloc(&dout.base, n_duplex_out + 8));
-    FGB_CUDA(h, pool.alloc(&dout.qual, n_duplex_out + 8));
-    FGB_CUDA(h, pool.alloc(&dout.errors, n_duplex_out + 8));
-    FGB_CUDA(h, pool.alloc(&dout.status, n_jobs));
-    FGB_CUDA(h, cudaMemcpyAsync(djobs, jobs, n_jobs * sizeof(fgb_duplex_job), cudaMemcpyHostToDevice, s));
-    if ((st = fgb_duplex_combine_device(h, &d.b, &d.ss, djobs, n_jobs, &dout, s)) != FGB_OK) return st;
-    FGB_CUDA(h, cudaMemcpyAsync(out->base, dout.base, n_duplex_out, cudaMemcpyDeviceToHost, s));
-    FGB_CUDA(h, cudaMemcpyAsync(out->qual, dout.qual, n_duplex_out, cudaMemcpyDeviceToHost, s));
-    FGB_CUDA(h, cudaMemcpyAsync(out->errors, dout.errors, n_duplex_out * 2, cudaMemcpyDeviceToHost, s));
-    if (out->status) FGB_CUDA(h, cudaMemcpyAsync(out->status, dout.status, n_jobs, cudaMemcpyDeviceToHost, s));
-  }
-  FGB_CUDA(h, cudaStreamSynchronize(s));
-  return FGB_OK;
-}
-
-fgb_status fgb_codec_submit(fgb_handle* h, const fgb_batch* in, const fgb_columns* ss_out,
-                            const fgb_codec_job* jobs, uint64_t n_jobs, const fgb_codec_params* cp,
-                            uint64_t n_codec_out, const fgb_codec_out* out) {
-  if (!h || !in || !ss_out || (n_jobs && (!jobs || !out || !cp))) return FGB_ERR_INVALID_ARG;
-  if (in->n_tiles == 0) return FGB_OK;
-  FGB_CUDA(h, cudaSetDevice(h->device));
-  cudaStream_t s = h->slots[0].stream;
-  DevPool pool;
-  DeviceBatchCopy d;
-  fgb_status st = upload_and_vote(h, in, &pool, &d, s);
-  if (st != FGB_OK) return st;
-  if ((st = download_ss(h, d, ss_out, in->n_out, s)) != FGB_OK) return st;
-  if (n_jobs) {
-    fgb_codec_job* djobs = nullptr;
-    fgb_codec_out dout{};
-    FGB_CUDA(h, pool.alloc(&djobs, n_jobs));
-    FGB_CUDA(h, pool.alloc(&dout.cols.base, n_codec_out + 8));
-    FGB_CUDA(h, pool.alloc(&dout.cols.qual, n_codec_out + 8));
-    FGB_CUDA(h, pool.alloc(&dout.cols.depth, n_codec_out + 8));
-    FGB_CUDA(h, pool.alloc(&dout.cols.errors, n_codec_out + 8));
-    FGB_CUDA(h, pool.alloc(&dout.status, n_jobs));
-    FGB_CUDA(h, pool.alloc(&dout.disagreements, n_jobs));
-    FGB_CUDA(h, pool.alloc(&dout.duplex_bases, n_jobs));
-    FGB_CUDA(h, cudaMemcpyAsync(djobs, jobs, n_jobs * sizeof(fgb_codec_job), cudaMemcpyHostToDevice, s));
-    if ((st = fgb_codec_combine_device(h, &d.b, &d.ss, djobs, n_jobs, cp, &dout, s)) != FGB_OK) return st;
-    FGB_CUDA(h, cudaMemcpyAsync(out->cols.base, dout.cols.base, n_codec_out, cudaMemcpyDeviceToHost, s));
-    FGB_CUDA(h, cudaMemcpyAsync(out->cols.qual, dout.cols.qual, n_codec_out, cudaMemcpyDeviceToHost, s));
-    FGB_CUDA(h, cudaMemcpyAsync(out->cols.depth, dout.cols.depth, n_codec_out * 2, cudaMemcpyDeviceToHost, s));
-    FGB_CUDA(h, cudaMemcpyAsync(out->cols.errors, dout.cols.errors, n_codec_out * 2, cudaMemcpyDeviceToHost, s));
-    FGB_CUDA(h, cudaMemcpyAsync(out->status, dout.status, n_jobs, cudaMemcpyDeviceToHost, s));
-    if (out->disagreements) FGB_CUDA(h, cudaMemcpyAsync(out->disagreements, dout.disagreements, n_jobs * 4, cudaMemcpyDeviceToHost, s));
-    if (out->duplex_bases) FGB_CUDA(h, cudaMemcpyAsync(out->duplex_bases, dout.duplex_bases, n_jobs * 4, cudaMemcpyDeviceToHost, s));
-  }
-  FGB_CUDA(h, cudaStreamSynchronize(s));
   return FGB_OK;
 }
 

@@ -23,6 +23,8 @@ constexpr uint32_t kTileMaxUnits = 127;    // unit descriptors per stage (16 B e
 #define FGB_WARP_QUEUE_CAP 96
 #endif
 constexpr uint32_t kWarpQueueCap = FGB_WARP_QUEUE_CAP;     // undecided positions buffered per warp per tile
+// shallow queues at least this long are resolved one position per lane, shorter ones eight lanes per position
+constexpr uint32_t kLaneMinQueue = 24u;
 constexpr uint32_t kQtEntries = 256;       // fast-path quality threshold table, indexed by min(n,255)
 
 constexpr uint32_t kTileFlagDirect = 1u;   // unit too large for a stage: kernel reads it from HBM

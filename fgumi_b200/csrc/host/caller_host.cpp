@@ -40,14 +40,6 @@ namespace {
 
 enum ReadType : uint8_t { kFragment = 0, kR1 = 1, kR2 = 2 };
 
-struct UnitMeta {                    // simplex: one per packed unit
-  uint8_t read_type;
-  std::string umi;
-  std::vector<std::string> rx;       // RX values of the surviving reads, in order
-  bool has_cell = false;
-  std::string cell;
-};
-
 struct RxSource {                    // duplex: one surviving raw read's RX + FIRST_SEGMENT flag
   std::string rx;
   bool first;
@@ -217,7 +209,6 @@ struct fgb_caller {
   PrepOptions prep_opt;
   uint64_t stats[FGB_NSTATS] = {0};
   Packer pack;
-  std::vector<UnitMeta> metas;           // simplex
   std::vector<Molecule> molecules;       // duplex
   std::vector<fgb_duplex_job> jobs;      // duplex
   uint64_t n_duplex_out = 0;
@@ -236,7 +227,6 @@ struct fgb_caller {
   std::vector<std::unique_ptr<fgb_caller>> workers;   // per-thread prep state of fgb_caller_add_groups (no GPU handle)
   std::unique_ptr<WorkerPool> pool;                    // the threads themselves, started on first use
   // flush scratch that outlives a flush, so steady-state flushes neither page-fault nor zero-fill:
-  std::vector<std::vector<uint8_t>> tbufs;   // per-thread record buffers (capacity kept)
   uint8_t* joined = nullptr;                 // output stream of a flush (page-locked, grow-only)
   size_t joined_cap = 0, joined_len = 0;
   bool out_is_joined = false;
@@ -363,24 +353,13 @@ void prepare_subgroup(fgb_caller* c, const std::vector<View>& recs, const std::v
   for (size_t i = 0; i < p->n; ++i) p->rec_idx.push_back(members[p->srs[i].original_idx]);
 }
 
-void pack_simplex_unit(fgb_caller* c, const std::vector<View>& recs, const Prepared& p, uint8_t read_type,
-                       const std::string& umi) {
-  c->pack.add_unit(p.srs, p.n, c->opt.min_reads);
-  UnitMeta m;
-  m.read_type = read_type;
-  m.umi = umi;
-  std::string s;
-  m.rx.reserve(p.rec_idx.size());
-  for (uint32_t ri : p.rec_idx) if (get_string_tag(recs[ri], "RX", &s)) m.rx.push_back(s);
-  if (c->opt.cell_tag[0] && !p.rec_idx.empty()) m.has_cell = get_string_tag(recs[p.rec_idx[0]], c->opt.cell_tag, &m.cell);
-  c->metas.push_back(std::move(m));
-}
+void pack_simplex_unit(fgb_caller* c, const Prepared& p) { c->pack.add_unit(p.srs, p.n, c->opt.min_reads); }
 
 // consensus_reads for one MI group (vanilla_caller.rs:1477-1499 + process_group :1042-1114).
 fgb_status add_group_simplex(fgb_caller* c, const std::vector<View>& recs) {
   const uint32_t n_records = static_cast<uint32_t>(recs.size());
-  std::string umi;
-  if (!get_string_tag(recs[0], c->opt.tag, &umi)) {   // vanilla_caller.rs:1493-1496
+  const uint8_t* uv; size_t un;
+  if (!bam::find_string_tag(recs[0], c->opt.tag, &uv, &un)) {   // vanilla_caller.rs:1493-1496
     c->last_error = std::string("Missing UMI tag '") + c->opt.tag[0] + c->opt.tag[1] + "'";
     return FGB_ERR_MISSING_TAG;
   }
@@ -415,12 +394,12 @@ fgb_status add_group_simplex(fgb_caller* c, const std::vector<View>& recs) {
   }
   Prepared &pf = c->prepared[0], &p1 = c->prepared[1], &p2 = c->prepared[2];   // pooled across groups
   prepare_subgroup(c, recs, frag, &pf);
-  if (pf.ok) { pack_simplex_unit(c, recs, pf, kFragment, umi); c->stats[FGB_STAT_CONSENSUS_READS] += 1; }
+  if (pf.ok) { pack_simplex_unit(c, pf); c->stats[FGB_STAT_CONSENSUS_READS] += 1; }
   prepare_subgroup(c, recs, r1, &p1);
   prepare_subgroup(c, recs, r2, &p2);
   if (p1.ok && p2.ok) {   // orphan rule, vanilla_caller.rs:1089-1108
-    pack_simplex_unit(c, recs, p1, kR1, umi);
-    pack_simplex_unit(c, recs, p2, kR2, umi);
+    pack_simplex_unit(c, p1);
+    pack_simplex_unit(c, p2);
     c->stats[FGB_STAT_CONSENSUS_READS] += 2;
   } else if (p1.ok) {
     reject(c, FGB_STAT_REJ_ORPHAN_CONSENSUS, p1.surviving);
@@ -718,173 +697,6 @@ struct PhaseTrace {
   }
 };
 
-// build_consensus_record_into, vanilla_caller.rs:1365-1473: one simplex consensus record from its columns.
-fgb_status write_simplex_record(const fgb_caller* c, bam::Writer* wp, const UnitMeta& m, uint32_t L,
-                                const uint8_t* bases, const uint8_t* quals, const uint16_t* depths,
-                                const uint16_t* errors, std::string* rx_scratch, std::string* err) {
-  bam::Writer& w = *wp;
-  std::string& rx = *rx_scratch;
-  uint16_t flag = bam::kUnmapped;
-  if (m.read_type == kR1) flag |= bam::kPaired | bam::kFirst | bam::kMateUnmapped;
-  else if (m.read_type == kR2) flag |= bam::kPaired | bam::kLast | bam::kMateUnmapped;
-  std::string name = c->prefix + ":" + m.umi;
-  if (name.size() >= 255) { *err = "read name too long"; return FGB_ERR_INVALID_ARG; }
-  w.begin(name, flag, bases, quals, L);
-  w.str("RG", c->rg.data(), c->rg.size());
-  uint32_t max_d = 0, min_d = L ? 0xFFFFFFFFu : 0;
-  uint64_t tot_e = 0, tot_d = 0;
-  for (uint32_t k = 0; k < L; ++k) {
-    max_d = std::max<uint32_t>(max_d, depths[k]);
-    min_d = std::min<uint32_t>(min_d, depths[k]);
-    tot_e += errors[k];
-    tot_d += depths[k];
-  }
-  w.integer("cD", static_cast<int32_t>(max_d));
-  w.integer("cM", static_cast<int32_t>(min_d));
-  w.real("cE", error_rate(tot_e, tot_d));
-  if (c->opt.produce_per_base_tags) {
-    w.i16_array("cd", depths, L);
-    w.i16_array("ce", errors, L);
-  }
-  w.str("MI", m.umi.data(), m.umi.size());
-  if (m.has_cell) w.str(c->opt.cell_tag, m.cell.data(), m.cell.size());
-  if (!m.rx.empty()) {
-    if (!consensus_umis(c->umi_builder, m.rx, &rx)) {   // the reference panics here (simple_umi.rs:78-116)
-      *err = "RX values of a family have different lengths or mix DNA and non-DNA characters";
-      return FGB_ERR_INVALID_ARG;
-    }
-    w.str("RX", rx.data(), rx.size());
-  }
-  return FGB_OK;
-}
-
-fgb_status flush_simplex(fgb_caller* c) {
-  const uint64_t U = c->pack.units.size();
-  if (!U) return FGB_OK;
-  PhaseTrace trace;
-  uint64_t n_bytes, R;
-  c->pack.seal(&n_bytes, &R);
-  uint64_t n_tiles = 0;
-  fgb_status st = fgb_plan_tiles(c->pack.units.data(), U, c->pack.reads.data(), R, nullptr, 0, &n_tiles);
-  if (st != FGB_OK) { c->last_error = "fgb_plan_tiles failed"; return st; }
-  std::vector<fgb_tile> tiles(n_tiles ? n_tiles : 1);
-  if ((st = fgb_plan_tiles(c->pack.units.data(), U, c->pack.reads.data(), R, tiles.data(), n_tiles, &n_tiles)) != FGB_OK) return st;
-  const uint64_t no = c->pack.n_out;
-  trace.mark("seal + plan");
-  if (c->pinned_cap < no + 8) {              // grow-only page-locked columns: no zero-fill, fast D2H
-    for (void*& p : c->pinned) { fgb_host_free(p); p = nullptr; }
-    c->pinned_cap = 0;
-    const size_t cap = (no + 8) + (no + 8) / 4;
-    const size_t bytes[4] = {cap, cap, cap * 2, cap * 2};
-    for (int i = 0; i < 4; ++i)
-      if (fgb_host_alloc(&c->pinned[i], bytes[i]) != FGB_OK) { c->last_error = "out of page-locked memory"; return FGB_ERR_NOMEM; }
-    c->pinned_cap = cap;
-  }
-  struct Col8 { uint8_t* p; uint8_t* data() const { return p; } };
-  struct Col16 { uint16_t* p; uint16_t* data() const { return p; } };
-  const Col8 ob{static_cast<uint8_t*>(c->pinned[0])}, oq{static_cast<uint8_t*>(c->pinned[1])};
-  const Col16 od{static_cast<uint16_t*>(c->pinned[2])}, oe{static_cast<uint16_t*>(c->pinned[3])};
-  trace.mark("output buffers");
-  fgb_batch b;
-  std::memset(&b, 0, sizeof(b));
-  b.n_units = U; b.n_reads = R; b.n_bytes = n_bytes; b.n_out = no; b.n_tiles = n_tiles;
-  b.bases = c->pack.bases.data(); b.quals = c->pack.quals.data(); b.reads = c->pack.reads.data();
-  b.units = c->pack.units.data(); b.tiles = tiles.data();
-  fgb_columns cols{ob.data(), oq.data(), od.data(), oe.data()};
-  std::vector<uint8_t> fstatus;
-  std::vector<uint32_t> fmasked;
-  if (c->opt.filter_enabled) {   // `fgumi filter` as an epilogue of the vote (commands/filter.rs:738-905)
-    fstatus.assign(U + 1, FGB_FILTER_PASS);
-    fmasked.assign(U + 1, 0);
-    fgb_filter_params fp = c->opt.filter;
-    fp.per_base_tags = c->opt.produce_per_base_tags;
-    fgb_submit_options so;
-    std::memset(&so, 0, sizeof(so));
-    so.input_format = FGB_IN_BYTES; so.output_format = FGB_OUT_U16;
-    so.filter = &fp; so.unit_status = fstatus.data(); so.unit_masked = fmasked.data();
-    st = fgb_submit_ex(c->h, &b, &cols, &so);
-  } else {
-    st = fgb_submit(c->h, &b, &cols);
-  }
-  if (st == FGB_OK) st = fgb_wait(c->h);
-  if (st != FGB_OK) {
-    char buf[256];
-    fgb_last_error(c->h, buf, sizeof(buf));
-    c->last_error = buf;
-    return st;
-  }
-  trace.mark("submit + wait");
-  // Template rule (commands/filter.rs:640-672): reads that share a name -- here the consecutive units
-  // of one MI -- are emitted only if every one of them passed.
-  std::vector<char> emit(U, 1);
-  if (c->opt.filter_enabled) {
-    for (uint64_t i = 0; i < U;) {
-      uint64_t j = i;
-      bool pass = true;
-      while (j < U && c->metas[j].umi == c->metas[i].umi) { pass = pass && fstatus[j] == FGB_FILTER_PASS; ++j; }
-      for (uint64_t k = i; k < j; ++k) {
-        emit[k] = pass;
-        c->stats[FGB_STAT_FILTER_RECORDS] += 1;
-        c->stats[FGB_STAT_FILTER_BASES_MASKED] += fmasked[k];
-        if (pass) c->stats[FGB_STAT_FILTER_PASSED] += 1;
-      }
-      i = j;
-    }
-  }
-  // ---- build_consensus_record_into, vanilla_caller.rs:1365-1473 ----
-  // Records are independent: with n_threads > 1 contiguous unit ranges are assembled into per-thread
-  // buffers and concatenated in order.
-  auto assemble = [&](uint64_t i0, uint64_t i1, std::vector<uint8_t>* dst, uint64_t* count,
-                      std::string* err) -> fgb_status {
-    bam::Writer w(dst);
-    std::string rx;
-    for (uint64_t i = i0; i < i1; ++i) {
-      if (!emit[i]) continue;
-      const fgb_unit& u = c->pack.units[i];
-      const UnitMeta& m = c->metas[i];
-      fgb_status rs = write_simplex_record(c, &w, m, u.cons_len, ob.data() + u.out_off, oq.data() + u.out_off,
-                                           od.data() + u.out_off, oe.data() + u.out_off, &rx, err);
-      if (rs != FGB_OK) return rs;
-      w.end();
-      ++*count;
-    }
-    return FGB_OK;
-  };
-  const uint32_t T = static_cast<uint32_t>(std::min<uint64_t>(std::max<uint32_t>(c->opt.n_threads, 1u), (U + 255) / 256));
-  if (T <= 1) {
-    std::string err;
-    st = assemble(0, U, &c->out, &c->out_count, &err);
-    if (st != FGB_OK) c->last_error = err;
-    trace.mark("assemble");
-    return st;
-  }
-  if (c->tbufs.size() < T) c->tbufs.resize(T);
-  std::vector<uint64_t> counts(T, 0);
-  std::vector<std::string> errs(T);
-  std::vector<fgb_status> sts(T, FGB_OK);
-  run_parallel(c, T, [&](uint32_t t) {
-    c->tbufs[t].clear();
-    sts[t] = assemble(U * t / T, U * (t + 1) / T, &c->tbufs[t], &counts[t], &errs[t]);
-  });
-  trace.mark("assemble (threads)");
-  size_t total = 0;
-  std::vector<size_t> at(T, 0);
-  for (uint32_t t = 0; t < T; ++t) {
-    if (sts[t] != FGB_OK) { c->last_error = errs[t]; return sts[t]; }
-    at[t] = total;
-    total += c->tbufs[t].size();
-    c->out_count += counts[t];
-  }
-  if (!ensure_joined(c, total)) return FGB_ERR_NOMEM;
-  run_parallel(c, T, [&](uint32_t t) {
-    if (!c->tbufs[t].empty()) std::memcpy(c->joined + at[t], c->tbufs[t].data(), c->tbufs[t].size());
-  });
-  c->joined_len = total;
-  c->out_is_joined = true;
-  trace.mark("concatenate");
-  return FGB_OK;
-}
-
 // ------------------------------------------------------------------------------------------------
 // simplex, direct path: flush
 // ------------------------------------------------------------------------------------------------
@@ -1092,8 +904,7 @@ fgb_status flush_simplex_direct(fgb_caller* c) {
   trace.mark("tiles");
   // ---- record assembly on the device (K5) when the engine offers it, every record's size is known up front (no
   //      unit deeper than 255 reads) and no filter decides what is emitted: the host supplies the strings only ----
-  static const bool kHostAssembly = std::getenv("FGB_CALLER_HOST_ASSEMBLY") != nullptr;
-  if (!kHostAssembly && !c->opt.filter_enabled && max_reads <= 255u && (fgb_engine_caps() & FGB_CAP_RECORD_ASSEMBLY)) {
+  if (!c->opt.filter_enabled && max_reads <= 255u && (fgb_engine_caps() & FGB_CAP_RECORD_ASSEMBLY)) {
     std::vector<uint64_t> rb_(NS + 1, 0), sb_(NS + 1, 0);
     const uint64_t head = c->prefix.size() + c->rg.size();
     sb_[0] = head;
@@ -2210,9 +2021,9 @@ static fgb_status caller_create_impl(int device, const fgb_caller_options* opt, 
   if (device != FGB_DEVICE_NONE) {       // FGB_DEVICE_NONE: planning only, flush refuses (no CPU fallback)
     fgb_status st = fgb_create(device, &p, &c->h);
     if (st != FGB_OK) return st;
-    // simplex callers with a device build the source-read rows on the device (FGB_CALLER_LEGACY=1 keeps the
-    // host decode; planning-only callers always use it, so the packed rows can be inspected)
-    c->direct = opt->mode == FGB_MODE_SIMPLEX && std::getenv("FGB_CALLER_LEGACY") == nullptr;
+    // simplex callers with a device build the source-read rows on the device (planning-only callers decode them
+    // on the host, so the packed rows can be inspected)
+    c->direct = opt->mode == FGB_MODE_SIMPLEX;
   }
   *out = c.release();
   return FGB_OK;
@@ -2328,7 +2139,6 @@ void merge_worker(fgb_caller* c, fgb_caller* w) {
   for (uint64_t d : w->pack.reads) c->pack.reads.push_back(FGB_READ_DESC(FGB_READ_OFF(d) + byte_base, FGB_READ_LEN(d)));
   for (fgb_unit u : w->pack.units) { u.out_off += out_base; u.read_begin += read_base; c->pack.units.push_back(u); }
   c->pack.n_out += w->pack.n_out;
-  for (auto& m : w->metas) c->metas.push_back(std::move(m));
   // duplex
   const int32_t job_base = static_cast<int32_t>(c->jobs.size());
   for (fgb_duplex_job j : w->jobs) { j.unit_a += unit_base; j.unit_b += unit_base; j.out_off += c->n_duplex_out; c->jobs.push_back(j); }
@@ -2351,7 +2161,7 @@ void merge_worker(fgb_caller* c, fgb_caller* w) {
   c->rejects.insert(c->rejects.end(), w->rejects.begin(), w->rejects.end());
   c->reject_count += w->reject_count;
   w->rejects.clear(); w->reject_count = 0;
-  w->pack.clear(); w->metas.clear(); w->molecules.clear(); w->jobs.clear();
+  w->pack.clear(); w->molecules.clear(); w->jobs.clear();
   w->codec_molecules.clear(); w->codec_jobs.clear();
   w->n_duplex_out = 0; w->n_codec_out = 0;
   std::memset(w->stats, 0, sizeof(w->stats));
@@ -2362,15 +2172,15 @@ void merge_worker(fgb_caller* c, fgb_caller* w) {
 // containers are sized once (the byte columns without zero-fill), every worker then writes its slice at
 // a precomputed offset with the same fix-ups merge_worker applies.  Byte-identical to the serial merge.
 void merge_workers_parallel(fgb_caller* c, uint32_t T) {
-  struct Base { size_t bytes, reads, units, metas, jobs, mols, cjobs, cmols; uint64_t out, dout, cout; };
+  struct Base { size_t bytes, reads, units, jobs, mols, cjobs, cmols; uint64_t out, dout, cout; };
   std::vector<Base> b(T + 1);
-  b[0] = Base{c->pack.bases.size(), c->pack.reads.size(), c->pack.units.size(), c->metas.size(), c->jobs.size(),
+  b[0] = Base{c->pack.bases.size(), c->pack.reads.size(), c->pack.units.size(), c->jobs.size(),
               c->molecules.size(), c->codec_jobs.size(), c->codec_molecules.size(), c->pack.n_out,
               c->n_duplex_out, c->n_codec_out};
   for (uint32_t t = 0; t < T; ++t) {
     const fgb_caller* w = c->workers[t].get();
     b[t + 1] = Base{b[t].bytes + w->pack.bases.size(), b[t].reads + w->pack.reads.size(), b[t].units + w->pack.units.size(),
-                    b[t].metas + w->metas.size(), b[t].jobs + w->jobs.size(), b[t].mols + w->molecules.size(),
+                    b[t].jobs + w->jobs.size(), b[t].mols + w->molecules.size(),
                     b[t].cjobs + w->codec_jobs.size(), b[t].cmols + w->codec_molecules.size(),
                     b[t].out + w->pack.n_out, b[t].dout + w->n_duplex_out, b[t].cout + w->n_codec_out};
   }
@@ -2378,7 +2188,6 @@ void merge_workers_parallel(fgb_caller* c, uint32_t T) {
   c->pack.quals.resize(b[T].bytes);
   c->pack.reads.resize(b[T].reads);
   c->pack.units.resize(b[T].units);
-  c->metas.resize(b[T].metas);
   c->jobs.resize(b[T].jobs);
   c->molecules.resize(b[T].mols);
   c->codec_jobs.resize(b[T].cjobs);
@@ -2399,7 +2208,6 @@ void merge_workers_parallel(fgb_caller* c, uint32_t T) {
       u.out_off += o.out; u.read_begin += static_cast<uint32_t>(o.reads);
       c->pack.units[o.units + i] = u;
     }
-    for (size_t i = 0; i < w->metas.size(); ++i) c->metas[o.metas + i] = std::move(w->metas[i]);
     for (size_t i = 0; i < w->jobs.size(); ++i) {
       fgb_duplex_job j = w->jobs[i];
       j.unit_a += static_cast<uint32_t>(o.units); j.unit_b += static_cast<uint32_t>(o.units); j.out_off += o.dout;
@@ -2437,7 +2245,7 @@ void merge_workers_parallel(fgb_caller* c, uint32_t T) {
     c->rejects.insert(c->rejects.end(), w->rejects.begin(), w->rejects.end());
     c->reject_count += w->reject_count;
     w->rejects.clear(); w->reject_count = 0;
-    w->pack.clear(); w->metas.clear(); w->molecules.clear(); w->jobs.clear();
+    w->pack.clear(); w->molecules.clear(); w->jobs.clear();
     w->codec_molecules.clear(); w->codec_jobs.clear();
     w->n_duplex_out = 0; w->n_codec_out = 0;
     std::memset(w->stats, 0, sizeof(w->stats));
@@ -2505,7 +2313,6 @@ fgb_status direct_add(fgb_caller* c, const uint8_t* records, const uint64_t* rec
       if (r1 < r0 || r1 - r0 > 0xFFFFFFFFull || r1 > rec1) { x->last_error = "bad group_rec table"; sts[t] = FGB_ERR_INVALID_ARG; return; }
       const uint32_t n = static_cast<uint32_t>(r1 - r0);
       if (n == 0) continue;
-#ifndef FGB_NO_RECORD_PREFETCH
       // The group rules read a record's fixed header, the start of its name / CIGAR and, at its end, the quality tail
       // and the aux area: three or four cache lines ~300 bytes apart per record, a miss each at DRAM latency.  Ask for
       // those lines of the NEXT group's records now (offsets beyond this worker's slice are simply not asked for).
@@ -2519,7 +2326,6 @@ fgb_status direct_add(fgb_caller* c, const uint8_t* records, const uint64_t* rec
           if (re - rp > 192) { __builtin_prefetch(re - 64, 0, 3); __builtin_prefetch(re - 128, 0, 3); }
         }
       }
-#endif
       x->views.clear();
       for (uint64_t r = r0; r < r1; ++r) {
         if (rec_off[r + 1] < rec_off[r] || rec_off[r + 1] > s1) { x->last_error = "record offsets must ascend"; sts[t] = FGB_ERR_LAYOUT; return; }
@@ -2695,7 +2501,7 @@ static fgb_status caller_flush_impl(fgb_caller* c, const uint8_t** out_data, uin
   }
   fgb_status st = c->opt.mode == FGB_MODE_DUPLEX ? flush_duplex(c)
                   : c->opt.mode == FGB_MODE_CODEC ? flush_codec(c)
-                  : c->direct ? flush_simplex_direct(c) : flush_simplex(c);
+                  : flush_simplex_direct(c);
   if (c->direct) {
     c->dplan.clear();
     for (auto& w : c->workers) w->dplan.clear();
@@ -2703,7 +2509,7 @@ static fgb_status caller_flush_impl(fgb_caller* c, const uint8_t** out_data, uin
     c->stage_len = 0;
     c->zc_base = nullptr;
   }
-  c->pack.clear(); c->metas.clear(); c->molecules.clear(); c->jobs.clear();
+  c->pack.clear(); c->molecules.clear(); c->jobs.clear();
   c->codec_molecules.clear(); c->codec_jobs.clear();
   c->n_duplex_out = 0; c->n_codec_out = 0;
   if (st != FGB_OK) return st;
@@ -2807,20 +2613,36 @@ fgb_status fgb_host_simplex_record(const char* read_name_prefix, const char* rea
   c.prefix = read_name_prefix;
   c.rg = read_group_id;
   c.opt.produce_per_base_tags = produce_per_base_tags ? 1 : 0;
-  UnitMeta m;
-  m.read_type = read_type == 0 ? kFragment : (read_type == 1 ? kR1 : kR2);
-  m.umi = umi;
-  if (cell_tag && cell) { c.opt.cell_tag[0] = cell_tag[0]; c.opt.cell_tag[1] = cell_tag[1]; m.has_cell = true; m.cell = cell; }
-  for (uint32_t i = 0; i < n_rx; ++i) { if (!rx[i]) return FGB_ERR_INVALID_ARG; m.rx.emplace_back(rx[i]); }
-  std::vector<uint8_t> buf;
-  bam::Writer w(&buf);
+  // the UMI, cell and RX strings in one buffer, referenced the way the flush references the staged records
+  std::string strs = umi;
+  DUnit u;
+  u.cons_len = len;
+  u.read_type = read_type;
+  u.umi = StrRef{0, static_cast<uint32_t>(strs.size())};
+  if (cell_tag && cell) {
+    c.opt.cell_tag[0] = cell_tag[0]; c.opt.cell_tag[1] = cell_tag[1];
+    u.has_cell = 1;
+    u.cell = StrRef{strs.size(), static_cast<uint32_t>(std::strlen(cell))};
+    strs += cell;
+  }
+  std::vector<StrRef> rx_refs;
+  for (uint32_t i = 0; i < n_rx; ++i) {
+    if (!rx[i]) return FGB_ERR_INVALID_ARG;
+    rx_refs.push_back(StrRef{strs.size(), static_cast<uint32_t>(std::strlen(rx[i]))});
+    strs += rx[i];
+  }
+  u.rx_n = n_rx;
+  uint32_t max_d = 0, min_d = len ? 0xFFFFFFFFu : 0u;
+  for (uint32_t k = 0; k < len; ++k) { max_d = std::max<uint32_t>(max_d, depths[k]); min_d = std::min<uint32_t>(min_d, depths[k]); }
+  const uint32_t size = simplex_record_size(&c, len, u.umi.len, u.has_cell, u.cell.len, n_rx > 0, n_rx ? rx_refs[0].len : 0u,
+                                            int_tag_width(max_d), int_tag_width(min_d));
+  if (size > cap) return FGB_ERR_INVALID_ARG;
   std::string scratch, err;
-  fgb_status st = write_simplex_record(&c, &w, m, len, bases, quals, depths, errors, &scratch, &err);
-  if (st != FGB_OK) return st;
-  w.end();
-  if (buf.size() > cap) return FGB_ERR_INVALID_ARG;
-  std::memcpy(out, buf.data(), buf.size());
-  *out_len = buf.size();
+  const size_t n = write_simplex_record_at<uint16_t>(&c, out, u, rx_refs.data(), reinterpret_cast<const uint8_t*>(strs.data()),
+                                                     bases, quals, depths, errors, &scratch, &err);
+  if (n == 0) return FGB_ERR_INVALID_ARG;      // read name too long, or RX values the reference rejects
+  if (n != size) return FGB_ERR_INVALID_ARG;   // simplex_record_size disagrees with the writer
+  *out_len = n;
   return FGB_OK;
 }
 

@@ -113,17 +113,7 @@ struct __align__(128) VoteSmem {
 
 constexpr uint32_t kPairSmemBytes = 94u * 94u;                 // 8836 = 4 * 2209
 constexpr uint32_t kUgapSmemOff = (kPairSmemBytes + 15u) & ~15u;   // the unanimous-gap steps follow the pair table
-// ... and behind them the shallow kernel's DEFERRED list: positions whose certified float evaluation
-// (certified_from_fixed) is put off until 32 of them can be evaluated one per lane (flush_deferred)
-constexpr uint32_t kDeferCap = 36u;            // a pass of the slow pass adds at most 4 to a list shorter than 32
-constexpr uint32_t kDeferWords = 5u;           // {global unit, pos << 16 | cw << 12 | depth << 8 | w << 1 | unanimous, g1, g2, g3}
-constexpr uint32_t kDeferSmemOff = kUgapSmemOff + 128u * 4u + 128u;
-#ifndef FGB_DEFER_CERT
-#define FGB_DEFER_CERT 0
-#endif
-constexpr uint32_t kDeferCountOff = kDeferSmemOff + (FGB_DEFER_CERT ? kConsumerWarps * kDeferCap * kDeferWords * 4u : 0u);
-constexpr uint32_t kShallowSmemBytes = kDeferCountOff + kConsumerWarps * 4u;
-static_assert(kDeferSmemOff % 4u == 0, "deferred entries are words");
+constexpr uint32_t kShallowSmemBytes = kUgapSmemOff + 128u * 4u + 128u;
 static_assert(kPairSmemBytes % 4u == 0, "pair table is copied as words");
 static_assert(sizeof(VoteSmem) % 16u == 0, "the pair table follows VoteSmem in dynamic shared memory");
 
@@ -257,12 +247,8 @@ __device__ __forceinline__ bool is_acgt_upper(uint32_t b) {
 // base do not reconverge before the end of the out-of-line resolver.
 __device__ __forceinline__ uint32_t base_to_index(uint32_t b) {
   const uint32_t u = b & 0xDFu;
-#ifdef FGB_B2I_BRANCHY
-  return u == 'A' ? 0u : u == 'C' ? 1u : u == 'G' ? 2u : u == 'T' ? 3u : 4u;
-#else
   const uint32_t x = (u >> 1) & 3u;            // A 0, C 1, T 2, G 3
   return is_acgt_upper(u) ? (x ^ (x >> 1)) : 4u;
-#endif
 }
 
 struct Called {
@@ -511,10 +497,6 @@ __device__ __forceinline__ uint32_t duplex_epilogue(const VoteArgsDuplex& a, con
   const uint32_t total = count * M;
   const uint32_t ub0 = st.tile.unit_begin;
   uint32_t done = 0;
-#ifndef FGB_EPI_MODE
-#define FGB_EPI_MODE 0      // A/B builds only (scripts/build_variants.sh): 1 barrier only, 2 no recount, 3 no SS read-back
-#endif
-  if (FGB_EPI_MODE == 1) return 0;
   for (uint32_t it = tid; it < total; it += kVoteThreads) {
     const uint32_t jl = it / M, p0 = (it - jl * M) * 8u;
     const uint32_t j = __ldg(a.job_index + jbegin + jl);
@@ -529,24 +511,17 @@ __device__ __forceinline__ uint32_t duplex_epilogue(const VoteArgsDuplex& a, con
     if ((out_off & 7ull) != 0ull || na + nb > 255u) continue;  // not a word-path job
     // :852-882 both strands must have coverage inside the truncated region; the first word nearly always shows it
     const uint32_t live0 = len < 8u ? len : 8u;
-#if FGB_EPI_MODE != 3
     const uint4 ad0 = __ldcg(reinterpret_cast<const uint4*>(a.out_depth + ua.out_off));
     const uint4 bd0 = __ldcg(reinterpret_cast<const uint4*>(a.out_depth + ub.out_off));
     if (!(duplex_any_depth(ad0, live0) && duplex_any_depth(bd0, live0))) continue;
-#endif
-#if FGB_EPI_MODE == 3
-    const uint2 ab2 = make_uint2(0x41414141u + p0, 0x43434343u), bb2 = make_uint2(0x41414141u + la, 0x43434343u);
-    const uint2 aq2 = make_uint2(0x1E1E1E1Eu, 0x1E1E1E1Eu), bq2 = aq2;
-#else
     const uint2 ab2 = __ldcg(reinterpret_cast<const uint2*>(a.out_base + ua.out_off + p0));
     const uint2 bb2 = __ldcg(reinterpret_cast<const uint2*>(a.out_base + ub.out_off + p0));
     const uint2 aq2 = __ldcg(reinterpret_cast<const uint2*>(a.out_qual + ua.out_off + p0));
     const uint2 bq2 = __ldcg(reinterpret_cast<const uint2*>(a.out_qual + ub.out_off + p0));
-#endif
     const DuplexWord w = duplex_combine_word(ab2, bb2, aq2, bq2);
     uint32_t cnt[2] = {0u, 0u};
     const uint32_t ra0 = ua.read_begin - read_base, rb0 = ub.read_begin - read_base;
-    const uint32_t nr = FGB_EPI_MODE == 2 ? 0u : na + nb;
+    const uint32_t nr = na + nb;
     for (uint32_t r0 = 0; r0 < nr; r0 += 4u) {                 // AB rows then BA rows, four in flight
       uint64_t d[4];
       uint2 sb[4];
@@ -718,92 +693,19 @@ __device__ __forceinline__ Called resolve_position(const TileView<M>& tv, const 
   return c;
 }
 
-// ---- deferred certified evaluation (shallow kernel) ---------------------------------------------------------
-// A shallow tile leaves each warp two or three positions with real dissent; evaluated where they are found, the
-// float tail of certified_from_fixed runs with two or three lanes active (a tenth of the kernel's instructions at
-// depth 4, and the warp that has them holds its tile's stage while the others wait).  Instead the slow pass parks
-// what the evaluation needs -- the three fixed-point gaps, the counts and where the result goes -- in a per-warp list
-// in shared memory, and the warp evaluates 32 parked positions at once, one per lane, whenever the list has that
-// many (and once more at the end of the kernel).  The position's word was stored by the fast pass of the same warp
-// long before (program order + __syncwarp), its bytes are overwritten here.  A position the certified evaluation
-// refuses goes to the literal f64 path reading its rows from global memory (the stage is gone).
-struct DeferCtx {                 // what flush_deferred needs of VoteArgs, by value (it is not inlined)
-  const uint8_t* bases; const uint8_t* quals; const uint64_t* reads; const fgb_unit* units;
-  uint8_t* out_base; uint8_t* out_qual; uint16_t* out_depth; uint16_t* out_errors;
-  uint32_t min_reads, min_cons_q, fast_qual;
-};
-__device__ __forceinline__ DeferCtx defer_ctx(const VoteArgs& a) {
-  DeferCtx c;
-  c.bases = a.bases; c.quals = a.quals; c.reads = a.reads; c.units = a.units;
-  c.out_base = a.out_base; c.out_qual = a.out_qual; c.out_depth = a.out_depth; c.out_errors = a.out_errors;
-  c.min_reads = a.min_reads; c.min_cons_q = a.min_cons_q; c.fast_qual = a.fast_qual;
-  return c;
-}
-// Warp-collective.  Returns (literal-path positions << 16) | no-call positions of this lane.
-__device__ __noinline__ uint32_t flush_deferred(const DeferCtx a, const VoteSmem& S, const uint32_t* dq,
-                                                uint32_t* dcount, const uint32_t lane) {
-  __syncwarp();
-  const uint32_t cnt = *dcount;
-  uint32_t stats = 0;
-  for (uint32_t e = lane; e < cnt; e += 32u) {
-    const uint32_t* ent = dq + e * kDeferWords;
-    const uint32_t ug = ent[0], pm = ent[1];
-    const int32_t g1 = static_cast<int32_t>(ent[2]), g2 = static_cast<int32_t>(ent[3]), g3 = static_cast<int32_t>(ent[4]);
-    const uint32_t pos = pm >> 16, cw = (pm >> 12) & 15u, depth = (pm >> 8) & 15u, w = (pm >> 1) & 3u;
-    const uint4 un = __ldg(reinterpret_cast<const uint4*>(a.units + ug));     // {out_off lo, hi, read_begin, cons_len}
-    const uint64_t o = ((static_cast<uint64_t>(un.y) << 32) | un.x) + pos;
-    Called c;
-    uint32_t q = a.fast_qual;
-    if (certified_from_fixed(0, -g1, -g2, -g3, depth, (pm & 1u) != 0u, S.ln_pre, a.fast_qual, &q)) {
-      c.depth = depth;
-      c.errors = depth - cw;
-      if (depth < a.min_reads) { c.base = 'N'; c.qual = 0; }
-      else if (q < a.min_cons_q) { c.base = 'N'; c.qual = 2; }
-      else { c.base = (0x54474341u >> (8u * w)) & 0xFFu; c.qual = q; }
-    } else {
-      const uint32_t rb = un.z;
-      const uint32_t n = __ldg(reinterpret_cast<const uint32_t*>(a.units + ug + 1) + 2) - rb;
-      TileView<GlMem> tv;
-      tv.bases = a.bases; tv.quals = a.quals;
-      tv.reads = reinterpret_cast<const uint8_t*>(a.reads + rb);
-      tv.byte_base = 0; tv.read_base = rb;
-      c = exact_position<GlMem>(tv, S, rb, n, pos, a.min_reads, a.min_cons_q, a.fast_qual);
-      stats += (c.depth >> 31) << 16;
-      c.depth &= ~kLiteralFlag;
-    }
-    stats += (c.base == 'N');
-    a.out_base[o] = static_cast<uint8_t>(c.base);
-    a.out_qual[o] = static_cast<uint8_t>(c.qual);
-    a.out_depth[o] = static_cast<uint16_t>(c.depth);
-    a.out_errors[o] = static_cast<uint16_t>(c.errors);
-  }
-  __syncwarp();
-  if (lane == 0) *dcount = 0;
-  __syncwarp();
-  return stats;
-}
-
 // Resolves a warp's queued positions.  The depth axis is split across a GROUP of lanes (8 lanes
 // per position when every queued pileup has <= 8 reads, else the whole warp): each lane classifies
 // its reads and looks up their fixed-point likelihood gaps, a __shfl_xor butterfly sums the four
 // per-base gap sums and counts over the group, and the group leader applies the dominant-winner
 // proof (host_tables.cpp).  Whatever the proof cannot decide runs the literal f64 algorithm.
-template <class M, uint32_t G, bool Cert = false, bool Defer = false>
+template <class M, uint32_t G, bool Cert = false>
 __device__ __forceinline__ void slow_pass_g(const VoteArgs& a, const VoteSmem& S, const Stage& st,
                                             const TileView<M>& tv, const uint32_t* wqueue, uint32_t qn,
-                                            uint32_t lane, LocalStats& ls, uint32_t* dq = nullptr,
-                                            uint32_t* dcount = nullptr) {
+                                            uint32_t lane, LocalStats& ls) {
   constexpr uint32_t per_pass = 32u / G;
   constexpr uint32_t gshift = G == 8u ? 3u : 5u;
   const uint32_t sub = lane & (G - 1u);
   for (uint32_t e0 = 0; e0 < qn; e0 += per_pass) {
-    if (Defer) {                                 // warp-uniform: the list is read after a __syncwarp
-      __syncwarp();
-      if (*dcount >= 32u) {
-        const uint32_t fs = flush_deferred(defer_ctx(a), S, dq, dcount, lane);
-        ls.exact += fs >> 16; ls.nocall += fs & 0xFFFFu;
-      }
-    }
     const uint32_t e = e0 + (lane >> gshift);
     const bool valid = e < qn;
     uint32_t u = 0, pos = 0, rb = 0, n = 0;
@@ -854,7 +756,6 @@ __device__ __forceinline__ void slow_pass_g(const VoteArgs& a, const VoteSmem& S
     if (valid && sub == 0) {
       Called c;
       bool done = false;
-      bool continue_pass = false;               // parked in the deferred list: nothing to write now
       if (provable) {
         const uint32_t c0 = c01 & 0xFFFFu, c1 = c01 >> 16, c2 = c23 & 0xFFFFu, c3 = (c23 >> 16) & 0x7FFFu;
         const uint32_t depth = c0 + c1 + c2 + c3;
@@ -873,16 +774,7 @@ __device__ __forceinline__ void slow_pass_g(const VoteArgs& a, const VoteSmem& S
                         static_cast<int64_t>(S.g2fix) + 2 * static_cast<int64_t>(depth) + 1;
           if (Cert && !proven) {
             const int32_t oa = w == 0 ? s1 : s0, ob = w <= 1 ? s2 : s1, oc = w == 3 ? s2 : s3;
-            if (Defer && depth <= 15u) {         // park it: evaluated 32 at a time by flush_deferred
-              uint32_t* ent = dq + atomicAdd(dcount, 1u) * kDeferWords;
-              ent[0] = st.tile.unit_begin + u;
-              ent[1] = (pos << 16) | (cw << 12) | (depth << 8) | (w << 1) | (depth == cw ? 1u : 0u);
-              ent[2] = static_cast<uint32_t>(best - oa); ent[3] = static_cast<uint32_t>(best - ob);
-              ent[4] = static_cast<uint32_t>(best - oc);
-              continue_pass = true;
-            } else {
-              proven = certified_from_fixed(best, oa, ob, oc, depth, depth == cw, S.ln_pre, a.fast_qual, &q);
-            }
+            proven = certified_from_fixed(best, oa, ob, oc, depth, depth == cw, S.ln_pre, a.fast_qual, &q);
           }
           if (proven) {
             c.depth = depth;
@@ -894,15 +786,13 @@ __device__ __forceinline__ void slow_pass_g(const VoteArgs& a, const VoteSmem& S
           }
         }
       }
-      if (!continue_pass) {
-        if (!done) {
-          c = exact_position<M>(tv, S, rb, n, pos, a.min_reads, a.min_cons_q, a.fast_qual);
-          ls.exact += c.depth >> 31;
-          c.depth &= ~kLiteralFlag;
-        }
-        ls.nocall += (c.base == 'N');
-        write_called(a, out_off + pos, c);
+      if (!done) {
+        c = exact_position<M>(tv, S, rb, n, pos, a.min_reads, a.min_cons_q, a.fast_qual);
+        ls.exact += c.depth >> 31;
+        c.depth &= ~kLiteralFlag;
       }
+      ls.nocall += (c.base == 'N');
+      write_called(a, out_off + pos, c);
     }
   }
 }
@@ -910,11 +800,10 @@ __device__ __forceinline__ void slow_pass_g(const VoteArgs& a, const VoteSmem& S
 // Group width (warp-uniform): 8 lanes per position (each lane strides the depth axis by 8) when no
 // queued pileup is deeper than 64 reads -- the planner's shallow-tile hint answers that without
 // looking -- else the whole warp per position.
-template <class M, bool Cert = false, bool Defer = false>
+template <class M, bool Cert = false>
 __device__ __forceinline__ void slow_pass(const VoteArgs& a, const VoteSmem& S, const Stage& st,
                                           const TileView<M>& tv, const uint32_t* wqueue, uint32_t qn,
-                                          uint32_t lane, LocalStats& ls, uint32_t* dq = nullptr,
-                                          uint32_t* dcount = nullptr) {
+                                          uint32_t lane, LocalStats& ls) {
   bool shallow = (st.tile.flags & kTileFlagShallow) != 0;
   if (!shallow) {
     uint32_t nmax = 0;
@@ -930,14 +819,8 @@ __device__ __forceinline__ void slow_pass(const VoteArgs& a, const VoteSmem& S, 
     }
     shallow = nmax <= 64u;
   }
-#ifndef FGB_SLOW_PER_LANE
-#define FGB_SLOW_PER_LANE 1
-#endif
-#ifndef FGB_LANE_MIN_QUEUE
-#define FGB_LANE_MIN_QUEUE 24u
-#endif
-  if (shallow && (!FGB_SLOW_PER_LANE || qn < FGB_LANE_MIN_QUEUE)) {
-    slow_pass_g<M, 8u, Cert, Defer>(a, S, st, tv, wqueue, qn, lane, ls, dq, dcount);
+  if (shallow && qn < kLaneMinQueue) {
+    slow_pass_g<M, 8u, Cert>(a, S, st, tv, wqueue, qn, lane, ls);
   } else if (shallow) {
     // one lane per queued position: with at most 64 reads the depth loop is short, and 32 positions
     // per pass beat splitting each pileup over a group of lanes
@@ -965,7 +848,7 @@ __device__ __forceinline__ void slow_pass(const VoteArgs& a, const VoteSmem& S, 
 // two-read units take the pair table in line.  (A sum-of-qualities proof for three- and four-read units was
 // built and measured: the exact threshold -- host_tables.cpp sumt -- has to guard against one very low
 // quality among high ones and ends up above what the per-read minimum test already accepts; dropped.)
-template <class M, bool Regular, int V = 0, bool Defer = false>
+template <class M, bool Regular, int V = 0>
 __device__ __forceinline__ void vote_tile(const VoteArgs& a, VoteSmem& S, const Stage& st,
                                           const TileView<M>& tv, uint32_t vt, uint32_t warp,
                                           uint32_t n_items, LocalStats& ls) {
@@ -1281,16 +1164,7 @@ __device__ __forceinline__ void vote_tile(const VoteArgs& a, VoteSmem& S, const 
   //  the warp + __syncwarp() orders the byte stores below after it)
   uint32_t qn = *wcount;
   qn = qn < kWarpQueueCap ? qn : kWarpQueueCap;
-  if (qn) {
-    if (Defer) {
-      uint8_t* const dyn = reinterpret_cast<uint8_t*>(&S) + sizeof(VoteSmem);
-      slow_pass<M, V == 1, true>(a, S, st, tv, wqueue, qn, lane, ls,
-                                 reinterpret_cast<uint32_t*>(dyn + kDeferSmemOff) + warp * (kDeferCap * kDeferWords),
-                                 reinterpret_cast<uint32_t*>(dyn + kDeferCountOff) + warp);
-    } else {
-      slow_pass<M, V == 1>(a, S, st, tv, wqueue, qn, lane, ls);
-    }
-  }
+  if (qn) slow_pass<M, V == 1>(a, S, st, tv, wqueue, qn, lane, ls);
   __syncwarp();
   if (lane == 0) *wcount = 0;
 }
@@ -1793,9 +1667,6 @@ __device__ __forceinline__ void vote_tile_deep_flat(const VoteArgs& a, VoteSmem&
   if (lane == 0) *wcount = 0;
 }
 
-#ifndef FGB_DEFER_CERT
-#define FGB_DEFER_CERT 0          // shallow kernel: certified evaluations parked and run 32 at a time (flush_deferred).
-#endif                            // Measured (gpurun iter7): depth 4 0.609 -> 0.621, depth 3 0.539 -> 0.494, depth 2 0.502 -> 0.437: off.
 #ifndef FGB_DEEP_FLAT_MIN
 #define FGB_DEEP_FLAT_MIN 64      // the flat deep form takes single-unit tiles of at least this many reads
 #endif
@@ -1815,8 +1686,6 @@ __device__ __forceinline__ void vote_kernel_body(const Args& a) {
   for (uint32_t i = tid; i < kQtEntries; i += kThreads) { S.qt[i] = a.tables->qt[i]; S.qt3[i] = a.tables->qt3[i]; }
   for (uint32_t i = tid; i < 96; i += kThreads) S.dfix[i] = a.tables->dfix[i];
   if (tid < kConsumerWarps) S.q_count[tid] = 0;
-  constexpr bool kDefer = V == 1 && !Fused && FGB_DEFER_CERT;   // (with the duplex epilogue a tile's results must be complete)
-  if (V == 1 && tid < kConsumerWarps) reinterpret_cast<uint32_t*>(smem_raw + sizeof(VoteSmem) + kDeferCountOff)[tid] = 0u;
   if (V == 1) {                                             // the shallow kernel's in-line pair table
     uint32_t* dst = reinterpret_cast<uint32_t*>(smem_raw + sizeof(VoteSmem));
     const uint32_t* src = reinterpret_cast<const uint32_t*>(a.tables->pair_q);
@@ -1961,7 +1830,7 @@ __device__ __forceinline__ void vote_kernel_body(const Args& a) {
       tv.reads = reinterpret_cast<const uint8_t*>(a.reads + st.tile.read_begin);
       tv.byte_base = 0; tv.read_base = st.tile.read_begin;
       if (V == 2) vote_tile_deep<GlMem, false>(a, S, st, tv, tid, warp, n_items, ls);
-      else vote_tile<GlMem, false, V, kDefer>(a, S, st, tv, vt, warp, n_items, ls);
+      else vote_tile<GlMem, false, V>(a, S, st, tv, vt, warp, n_items, ls);
     } else {
       TileView<ShMem> tv;
       tv.bases = st.bases; tv.quals = st.quals;
@@ -1977,8 +1846,8 @@ __device__ __forceinline__ void vote_kernel_body(const Args& a) {
         } else if (st.tile.flags & kTileFlagRegular) vote_tile_deep<ShMem, true>(a, S, st, tv, tid, warp, n_items, ls);
         else vote_tile_deep<ShMem, false>(a, S, st, tv, tid, warp, n_items, ls);
       } else {
-        if (st.tile.flags & kTileFlagRegular) vote_tile<ShMem, true, V, kDefer>(a, S, st, tv, vt, warp, n_items, ls);
-        else vote_tile<ShMem, false, V, kDefer>(a, S, st, tv, vt, warp, n_items, ls);
+        if (st.tile.flags & kTileFlagRegular) vote_tile<ShMem, true, V>(a, S, st, tv, vt, warp, n_items, ls);
+        else vote_tile<ShMem, false, V>(a, S, st, tv, vt, warp, n_items, ls);
       }
       if constexpr (Fused) {
         const uint2 tj = __ldg(reinterpret_cast<const uint2*>(a.tile_jobs + t));   // {begin, count | max_items << 16}
@@ -2015,12 +1884,6 @@ __device__ __forceinline__ void vote_kernel_body(const Args& a) {
   }
 #endif
 
-  if (kDefer) {                                             // what is still parked
-    const uint32_t fs = flush_deferred(defer_ctx(a), S,
-                                       reinterpret_cast<const uint32_t*>(smem_raw + sizeof(VoteSmem) + kDeferSmemOff) + warp * (kDeferCap * kDeferWords),
-                                       reinterpret_cast<uint32_t*>(smem_raw + sizeof(VoteSmem) + kDeferCountOff) + warp, tid & 31u);
-    ls.exact += fs >> 16; ls.nocall += fs & 0xFFFFu;
-  }
   // ---- counters: warp-reduce, one atomic per warp ----
   uint32_t v0 = ls.positions, v1 = ls.exact, v2 = ls.nocall;
 #pragma unroll

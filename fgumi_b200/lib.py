@@ -208,7 +208,7 @@ SYMBOLS = (
     "fgb_plan_tiles", "fgb_plan_tiles_jobs", "fgb_sort_tiles_by_class", "fgb_vote_device", "fgb_vote_duplex_device", "fgb_submit", "fgb_wait", "fgb_host_alloc",
     "fgb_host_free", "fgb_host_is_pinned", "fgb_duplex_combine_device", "fgb_codec_combine_device", "fgb_stats",
     "fgb_stats_device_ptr", "fgb_stats_reset", "fgb_launch_count", "fgb_engine_caps",
-    "fgb_duplex_submit", "fgb_codec_submit", "fgb_caller_create", "fgb_caller_destroy", "fgb_caller_last_error", "fgb_caller_add_group",
+    "fgb_caller_create", "fgb_caller_destroy", "fgb_caller_last_error", "fgb_caller_add_group",
     "fgb_caller_flush", "fgb_caller_take_rejects", "fgb_caller_stats", "fgb_overlap_apply_group", "fgb_pack8_encode",
     "fgb_submit_pack8", "fgb_submit_bam4", "fgb_unpack_bam4_device", "fgb_unpack_records_device", "fgb_submit_ex", "fgb_filter_simplex_device", "fgb_struct_size", "fgb_caller_add_groups", "fgb_filter_record", "fgb_host_is_fr_pair",
     "fgb_host_num_bases_extending_past_mate", "fgb_host_clip_cigar_ops", "fgb_host_read_pos_at_ref_pos", "fgb_host_simplify_cigar", "fgb_host_source_reads", "fgb_host_consensus_umis", "fgb_caller_pending", "fgb_host_simplex_record", "fgb_bgzf_bound", "fgb_bgzf_compress", "fgb_bgzf_scan_members", "fgb_bgzf_inflate_device", "fgb_host_inflate_member", "fgb_bam_header", "fgb_bgzf_uncompressed_size", "fgb_bgzf_decompress", "fgb_bam_read_header", "fgb_bam_split_records", "fgb_host_group_by_mi", "fgb_host_duplex_record",
@@ -295,12 +295,6 @@ def load() -> C.CDLL:
                                              u64, C.POINTER(FgbCodecParams),
                                              C.POINTER(FgbCodecOut), vp]
     lib.fgb_codec_combine_device.restype = C.c_int32
-    lib.fgb_duplex_submit.argtypes = [vp, C.POINTER(FgbBatch), C.POINTER(FgbColumns), vp, u64, u64,
-                                      C.POINTER(FgbDuplexOut)]
-    lib.fgb_duplex_submit.restype = C.c_int32
-    lib.fgb_codec_submit.argtypes = [vp, C.POINTER(FgbBatch), C.POINTER(FgbColumns), vp, u64,
-                                     C.POINTER(FgbCodecParams), u64, C.POINTER(FgbCodecOut)]
-    lib.fgb_codec_submit.restype = C.c_int32
     lib.fgb_stats.argtypes = [vp, C.POINTER(u64)]
     lib.fgb_stats.restype = C.c_int32
     lib.fgb_stats_device_ptr.argtypes = [vp, C.POINTER(vp)]

@@ -45,7 +45,7 @@
 extern "C" {
 #endif
 
-#define FGB_ABI_VERSION 3
+#define FGB_ABI_VERSION 4
 #define FGB_READ_ALIGN 8u   /* byte alignment of every read row in bases[]/quals[]          */
 #define FGB_OUT_ALIGN 8u    /* element alignment of every unit's output row                 */
 #define FGB_MAX_READ_LEN 65535u
@@ -598,18 +598,6 @@ fgb_status fgb_codec_combine_device(fgb_handle* h, const fgb_batch* in, const fg
                                     const fgb_codec_job* jobs, uint64_t n_jobs,
                                     const fgb_codec_params* cp, const fgb_codec_out* out,
                                     void* stream);
-
-/* Host-buffer forms of vote + strand combine (what the duplex / CODEC callers use): every pointer
- * is a HOST pointer.  One shot and synchronous: the batch is copied to the device, voted, combined,
- * and BOTH the single-strand columns (`ss_out`, needed for the ac/ad/ae/aq, bc/bd/be/bq tags) and the
- * combined columns are copied back before the call returns.  n_*_out = elements in each combined
- * output column. */
-fgb_status fgb_duplex_submit(fgb_handle* h, const fgb_batch* in, const fgb_columns* ss_out,
-                             const fgb_duplex_job* jobs, uint64_t n_jobs, uint64_t n_duplex_out,
-                             const fgb_duplex_out* out);
-fgb_status fgb_codec_submit(fgb_handle* h, const fgb_batch* in, const fgb_columns* ss_out,
-                            const fgb_codec_job* jobs, uint64_t n_jobs, const fgb_codec_params* cp,
-                            uint64_t n_codec_out, const fgb_codec_out* out);
 
 /* ---- simplex record assembly on the device (K5) ------------------------------------------------------
  * build_consensus_record_into (vanilla_caller.rs:1365-1473) for the units of a batch, written by the device at

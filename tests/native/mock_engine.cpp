@@ -1,10 +1,9 @@
 // TEST INFRASTRUCTURE -- NOT PRODUCT CODE.  A stand-in for the GPU engine behind the record-level callers,
 // so that the callers' flush side (tile planning, submit, record assembly, filter template rule, threaded
 // assembly) can run on a machine without a GPU and under sanitizers.  It defines the engine entry points
-// caller_host.cpp calls -- fgb_create / fgb_submit / fgb_submit_ex / fgb_wait / fgb_duplex_submit /
-// fgb_codec_submit / fgb_host_alloc ... -- on top of the CPU oracle (oracle/fgumi_oracle.cpp), and is
-// linked ONLY into tests/native/caller_e2e.cpp (the executable's definitions take precedence over the
-// library's).  The product has no CPU path: libfgumi_b200.so never contains or loads any of this.
+// caller_host.cpp calls -- fgb_create / fgb_submit / fgb_submit_ex / fgb_wait / fgb_host_alloc ... -- on
+// top of the CPU oracle (oracle/fgumi_oracle.cpp), and is linked ONLY into tests/native/caller_e2e.cpp
+// (the executable's definitions take precedence over the library's).  The product has no CPU path: libfgumi_b200.so never contains or loads any of this.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -247,14 +246,6 @@ static void run_duplex_jobs(const fgb_batch* in, const fgb_columns* ss, const fg
   }
 }
 
-fgb_status fgb_duplex_submit(fgb_handle* h, const fgb_batch* in, const fgb_columns* ss, const fgb_duplex_job* jobs,
-                             uint64_t n_jobs, uint64_t, const fgb_duplex_out* out) {
-  fgb_status st = vote(h, in, ss);
-  if (st != FGB_OK) return st;
-  run_duplex_jobs(in, ss, jobs, n_jobs, out);
-  return FGB_OK;
-}
-
 static void run_codec_jobs(const fgb_batch* in, const fgb_columns* ss, const fgb_codec_job* jobs, uint64_t n_jobs,
                            const fgb_codec_params* cp, const fgb_codec_out* out) {
   for (uint64_t j = 0; j < n_jobs; ++j) {
@@ -274,14 +265,6 @@ static void run_codec_jobs(const fgb_batch* in, const fgb_columns* ss, const fgb
     if (out->disagreements) out->disagreements[j] = static_cast<uint32_t>(dis);
     if (out->duplex_bases) out->duplex_bases[j] = static_cast<uint32_t>(dup);
   }
-}
-
-fgb_status fgb_codec_submit(fgb_handle* h, const fgb_batch* in, const fgb_columns* ss, const fgb_codec_job* jobs,
-                            uint64_t n_jobs, const fgb_codec_params* cp, uint64_t, const fgb_codec_out* out) {
-  fgb_status st = vote(h, in, ss);
-  if (st != FGB_OK) return st;
-  run_codec_jobs(in, ss, jobs, n_jobs, cp, out);
-  return FGB_OK;
 }
 
 }  // extern "C"
