@@ -176,7 +176,7 @@ fgb_status launch_vote(fgb_handle* h, const fgb_batch& b, const fgb_columns& out
       const VoteArgs& v = x;
       if (cls == 1) vote_kernel_shallow<<<grid, kThreads, sizeof(VoteSmem) + kShallowSmemBytes, stream>>>(v);
       else if (cls == 2) vote_kernel_deep<<<grid, kThreads, sizeof(VoteSmem) + kDeepSmemBytes, stream>>>(v);
-      else vote_kernel<<<grid, kThreads, sizeof(VoteSmem), stream>>>(v);
+      else vote_kernel<<<grid, kThreads, sizeof(VoteSmem) + kPileSmemBytes, stream>>>(v);
     }
     h->launches++;
   };
@@ -293,7 +293,7 @@ fgb_status fgb_create(int device, const fgb_params* params, fgb_handle** out) {
   if ((e = cudaMemset(h->d_counters, 0, sizeof(unsigned long long) * FGB_NCOUNTERS)) != cudaSuccess)
     return fail(e, "cudaMemset counters");
   if ((e = cudaFuncSetAttribute(vote_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                static_cast<int>(sizeof(VoteSmem)))) != cudaSuccess)
+                                static_cast<int>(sizeof(VoteSmem) + kPileSmemBytes))) != cudaSuccess)
     return fail(e, "cudaFuncSetAttribute(vote_kernel)");
   if ((e = cudaFuncSetAttribute(vote_kernel_shallow, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(sizeof(VoteSmem) + kShallowSmemBytes))) != cudaSuccess)

@@ -116,6 +116,8 @@ constexpr uint32_t kUgapSmemOff = (kPairSmemBytes + 15u) & ~15u;   // the unanim
 constexpr uint32_t kShallowSmemBytes = kUgapSmemOff + 128u * 4u + 128u;
 static_assert(kPairSmemBytes % 4u == 0, "pair table is copied as words");
 static_assert(sizeof(VoteSmem) % 16u == 0, "the pair table follows VoteSmem in dynamic shared memory");
+// Two CTAs per SM: 228 KiB of shared memory per SM, 1 KiB of it reserved per CTA.
+constexpr uint32_t kSmemPerCtaMax = 228u * 1024u / 2u - 1024u;
 
 // ---- PTX wrappers ------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -190,10 +192,33 @@ __device__ __forceinline__ void tma_load_1d(void* dst, const void* src, uint32_t
 // [0] CTA cycles (producer lane, prologue to last issue)  [1] producer cycles waiting on `empty`
 // [2] consumer-warp cycles  [3] consumer cycles waiting on `full`  [4] voting cycles  [5] fast pass  [6] slow pass
 // [7] tiles whose copy had not landed when warp 0 arrived  [8] their issue -> full cycles  [9] tiles  [10] CTAs
+// [11] stage hold: warp 0 passing `full` -> the last warp's arrival on `empty`  [12] last minus first arrival on `empty`
 constexpr int kPipeTraceWords = 16;
 __device__ unsigned long long g_pipe_trace[kPipeTraceWords];
 __shared__ long long g_trace_mark[kConsumerWarps];   // per warp: end of the fast pass of the current tile
+// per stage: when warp 0 passed `full`, first and last arrival on `empty`, arrivals so far
+__shared__ long long g_trace_full0[kStages];
+__shared__ unsigned long long g_trace_arr_first[kStages], g_trace_arr_last[kStages];
+__shared__ uint32_t g_trace_arr_n[kStages];
 #endif
+
+// Lane 0 of a consumer warp: this warp is done with stage s.
+__device__ __forceinline__ void release_stage(VoteSmem& S, int s) {
+#if FGB_PIPE_TRACE
+  const unsigned long long now = static_cast<unsigned long long>(clock64());
+  atomicMin(&g_trace_arr_first[s], now);
+  atomicMax(&g_trace_arr_last[s], now);
+  __threadfence_block();
+  if (atomicAdd(&g_trace_arr_n[s], 1u) == kConsumerWarps - 1u) {   // the last arrival: every warp's stamps are in
+    __threadfence_block();
+    const unsigned long long first = g_trace_arr_first[s], last = g_trace_arr_last[s];
+    atomicAdd(&g_pipe_trace[11], last - static_cast<unsigned long long>(g_trace_full0[s]));
+    atomicAdd(&g_pipe_trace[12], last - first);
+    g_trace_arr_first[s] = ~0ull; g_trace_arr_last[s] = 0ull; g_trace_arr_n[s] = 0u;   // before the stage can refill
+  }
+#endif
+  mbar_arrive(&S.empty[s]);
+}
 
 // ---- memory-space policy: tiles live in shared memory, oversize units are read from HBM -------
 struct ShMem {
@@ -365,20 +390,61 @@ __device__ __noinline__ bool certified_from_fixed(int32_t best, int32_t o1, int3
 // Bit 31 of the returned depth flags a result of the f64 algorithm (diagnostic counter).
 constexpr uint32_t kLiteralFlag = 0x80000000u;
 
+// Where the observations of one undecided position come from.  The resolvers below are written once against this
+// interface: `ref` and `n_reads` are the position's unit, `at` gives the row of observation r, or false when that
+// read does not cover the position.
+//   StageObs<M>: the unit's rows in the stage (or in HBM), through the read descriptors; ref = the unit's first read.
+//   PileObs:     a warp's pileup slot (gather_piles): the bytes of the covering reads only, in read order; ref = their
+//                count.  Dropping the uncovered reads changes nothing: the reference skips them (vanilla_caller.rs:1323).
 template <class M>
-__device__ __noinline__ Called exact_position(const TileView<M>& tv, const VoteSmem& S,
-                                              uint32_t read_begin, uint32_t n_reads,
+struct StageObs {
+  using view_t = TileView<M>;
+  using off_t = typename M::off_t;
+  static __device__ __forceinline__ uint32_t count(uint32_t, uint32_t n_reads) { return n_reads; }
+  static __device__ __forceinline__ bool at(const view_t& tv, uint32_t read_begin, uint32_t pos, uint32_t r, off_t& row) {
+    const uint64_t d = M::ld64(tv.reads + static_cast<off_t>(read_begin - tv.read_base + r) * 8u);
+    row = static_cast<off_t>((d >> 16) - tv.byte_base) + pos;
+    return pos < (static_cast<uint32_t>(d) & 0xFFFFu);
+  }
+  static __device__ __forceinline__ uint32_t base(const view_t& tv, off_t row) { return M::ld8(tv.bases + row); }
+  static __device__ __forceinline__ uint32_t qual(const view_t& tv, off_t row) { return M::ld8(tv.quals + row); }
+};
+
+// Pileup slot: [0, 8) output index, [8, 12) observations | reads << 16, then the observations' base and quality
+// bytes.  Every general-class unit (5..23 reads) fits a slot.
+constexpr uint32_t kPileMaxObs = 24u;
+constexpr uint32_t kPileSlotBytes = 64u;
+constexpr uint32_t kPileBases = 16u, kPileQuals = kPileBases + kPileMaxObs;
+constexpr uint32_t kPileSlots = 16u;                                  // per warp
+constexpr uint32_t kPileSmemBytes = kConsumerWarps * kPileSlots * kPileSlotBytes;
+static_assert(kPileQuals + kPileMaxObs <= kPileSlotBytes, "a slot holds kPileMaxObs observations");
+static_assert(sizeof(VoteSmem) + kPileSmemBytes <= kSmemPerCtaMax, "the general kernel must fit twice per SM");
+
+struct PileObs {
+  using view_t = const uint8_t*;
+  using off_t = uint32_t;
+  static __device__ __forceinline__ uint32_t count(uint32_t n_obs, uint32_t) { return n_obs; }
+  static __device__ __forceinline__ bool at(const view_t&, uint32_t n_obs, uint32_t, uint32_t r, off_t& row) {
+    row = r;
+    return r < n_obs;
+  }
+  static __device__ __forceinline__ uint32_t base(const view_t& p, off_t row) { return p[kPileBases + row]; }
+  static __device__ __forceinline__ uint32_t qual(const view_t& p, off_t row) { return p[kPileQuals + row]; }
+};
+
+template <class Src>
+__device__ __noinline__ Called exact_position(const typename Src::view_t& v, const VoteSmem& S,
+                                              uint32_t ref, uint32_t n_reads,
                                               uint32_t pos, uint32_t min_reads,
                                               uint32_t min_cons_q, uint32_t fast_qual) {
+  using off_t = typename Src::off_t;
   if (n_reads == 2u) {
-    const uint64_t d0 = M::ld64(tv.reads + static_cast<typename M::off_t>(read_begin - tv.read_base) * 8u);
-    const uint64_t d1 = M::ld64(tv.reads + static_cast<typename M::off_t>(read_begin - tv.read_base + 1u) * 8u);
-    if (pos < (static_cast<uint32_t>(d0) & 0xFFFFu) && pos < (static_cast<uint32_t>(d1) & 0xFFFFu)) {
-      const typename M::off_t r0 = static_cast<typename M::off_t>((d0 >> 16) - tv.byte_base) + pos;
-      const typename M::off_t r1 = static_cast<typename M::off_t>((d1 >> 16) - tv.byte_base) + pos;
-      const uint32_t i0 = base_to_index(M::ld8(tv.bases + r0));
-      if (i0 < 4u && i0 == base_to_index(M::ld8(tv.bases + r1))) {
-        uint32_t qa = M::ld8(tv.quals + r0), qb = M::ld8(tv.quals + r1);
+    off_t r0, r1;
+    const bool c0 = Src::at(v, ref, pos, 0u, r0), c1 = Src::at(v, ref, pos, 1u, r1);
+    if (c0 && c1) {
+      const uint32_t i0 = base_to_index(Src::base(v, r0));
+      if (i0 < 4u && i0 == base_to_index(Src::base(v, r1))) {
+        uint32_t qa = Src::qual(v, r0), qb = Src::qual(v, r1);
         qa = qa > FGB_MAX_PHRED ? FGB_MAX_PHRED : qa;
         qb = qb > FGB_MAX_PHRED ? FGB_MAX_PHRED : qb;
         const uint32_t cq = __ldg(S.pair_q + qa * 94u + qb);
@@ -396,15 +462,13 @@ __device__ __noinline__ Called exact_position(const TileView<M>& tv, const VoteS
   double ll[4] = {0.0, 0.0, 0.0, 0.0};   // LN_ONE
   double kc[4] = {0.0, 0.0, 0.0, 0.0};   // Kahan compensations
   uint64_t cnt = 0;                      // 4 x u16 observation counters
-  for (uint32_t r = 0; r < n_reads; ++r) {
-    uint64_t d = M::ld64(tv.reads + static_cast<typename M::off_t>(read_begin - tv.read_base + r) * 8u);
-    uint32_t len = static_cast<uint32_t>(d & 0xFFFFu);
-    if (pos < len) {                                          // vanilla_caller.rs:1323
-      typename M::off_t row = static_cast<typename M::off_t>((d >> 16) - tv.byte_base) + pos;
-      uint32_t b = M::ld8(tv.bases + row);
+  for (uint32_t r = 0; r < Src::count(ref, n_reads); ++r) {
+    off_t row;
+    if (Src::at(v, ref, pos, r, row)) {                       // vanilla_caller.rs:1323
+      uint32_t b = Src::base(v, row);
       uint32_t idx = base_to_index(b);
       if (b != 'N' && idx < 4u) {                             // :1328 and base_builder.rs:300
-        uint32_t q = M::ld8(tv.quals + row);
+        uint32_t q = Src::qual(v, row);
         q = q > FGB_MAX_PHRED ? FGB_MAX_PHRED : q;            // base_builder.rs:307
         double c = S.correct[q];
         double e = S.err_alt[q];
@@ -685,12 +749,95 @@ __device__ __forceinline__ Called resolve_position(const TileView<M>& tv, const 
                                                    const VoteArgs& a, LocalStats& ls) {
   Called c;
   if (!dominant_position<M, Cert>(tv, S, rb, n, pos, a.min_reads, a.min_cons_q, a.fast_qual, c)) {
-    c = exact_position<M>(tv, S, rb, n, pos, a.min_reads, a.min_cons_q, a.fast_qual);
+    c = exact_position<StageObs<M>>(tv, S, rb, n, pos, a.min_reads, a.min_cons_q, a.fast_qual);
     ls.exact += c.depth >> 31;
     c.depth &= ~kLiteralFlag;
   }
   ls.nocall += (c.base == 'N');
   return c;
+}
+
+// One pass of the group resolver: this lane's group votes one position (`valid`), whose observations `Src` gives;
+// the result goes to output index out_off + pos.
+template <class Src, uint32_t G, bool Cert>
+__device__ __forceinline__ void resolve_group(const VoteArgs& a, const VoteSmem& S, const typename Src::view_t& v,
+                                              bool valid, uint32_t ref, uint32_t n, uint32_t pos, uint64_t out_off,
+                                              uint32_t sub, LocalStats& ls) {
+  const bool provable = n <= S.nmax2;
+  int32_t s0 = 0, s1 = 0, s2 = 0, s3 = 0;
+  uint32_t c01 = 0, c23 = 0;      // 4 x u16 observation counts; bit 31 of c23 = "unusable quality seen"
+  if (provable) {
+    for (uint32_t r = sub; r < Src::count(ref, n); r += G) {
+      typename Src::off_t row;
+      if (Src::at(v, ref, pos, r, row)) {
+        uint32_t b = Src::base(v, row);
+        uint32_t q = Src::qual(v, row);
+        if (is_acgt_upper(b & 0xDFu)) {       // A,C,G,T in either case; 'N' and the rest are skipped
+          const uint32_t x = (b >> 1) & 3u;   // A 0, C 1, T 2, G 3
+          const uint32_t idx = x ^ (x >> 1);  // A 0, C 1, G 2, T 3
+          q = q > FGB_MAX_PHRED ? FGB_MAX_PHRED : q;
+          int32_t dq = S.dfix[q];
+          if (dq == INT32_MIN) { c23 |= 0x80000000u; dq = 0; }
+          s0 += idx == 0 ? dq : 0; s1 += idx == 1 ? dq : 0;
+          s2 += idx == 2 ? dq : 0; s3 += idx == 3 ? dq : 0;
+          c01 += idx == 0 ? 1u : (idx == 1 ? 0x10000u : 0u);
+          c23 += idx == 2 ? 1u : (idx == 3 ? 0x10000u : 0u);
+        }
+      }
+    }
+  }
+  // butterfly over the group (n <= nmax2 <= 1024 keeps every 16-bit count and the flag intact)
+#pragma unroll
+  for (uint32_t off = G >> 1; off > 0; off >>= 1) {
+    s0 += __shfl_xor_sync(0xFFFFFFFFu, s0, off);
+    s1 += __shfl_xor_sync(0xFFFFFFFFu, s1, off);
+    s2 += __shfl_xor_sync(0xFFFFFFFFu, s2, off);
+    s3 += __shfl_xor_sync(0xFFFFFFFFu, s3, off);
+    c01 += __shfl_xor_sync(0xFFFFFFFFu, c01, off);
+    uint32_t o23 = __shfl_xor_sync(0xFFFFFFFFu, c23, off);
+    c23 = ((c23 & 0x7FFFFFFFu) + (o23 & 0x7FFFFFFFu)) | ((c23 | o23) & 0x80000000u);
+  }
+  if (valid && sub == 0) {
+    Called c;
+    bool done = false;
+    if (provable) {
+      const uint32_t c0 = c01 & 0xFFFFu, c1 = c01 >> 16, c2 = c23 & 0xFFFFu, c3 = (c23 >> 16) & 0x7FFFu;
+      const uint32_t depth = c0 + c1 + c2 + c3;
+      if (depth == 0) {   // base_builder.rs:392-394 then vanilla_caller.rs:1345 (min_reads >= 1)
+        c.base = 'N'; c.qual = 0; c.depth = 0; c.errors = 0;
+        done = true;
+      } else if (!(c23 & 0x80000000u)) {
+        int32_t best = s0, second = INT32_MIN;
+        uint32_t w = 0, cw = c0;
+        if (s1 > best) { second = best; best = s1; w = 1; cw = c1; } else if (s1 > second) second = s1;
+        if (s2 > best) { second = best; best = s2; w = 2; cw = c2; } else if (s2 > second) second = s2;
+        if (s3 > best) { second = best; best = s3; w = 3; cw = c3; } else if (s3 > second) second = s3;
+        // every fixed-point term is within half a unit of D[q]*65536; two sums of <= depth terms
+        uint32_t q = a.fast_qual;
+        bool proven = static_cast<int64_t>(best) - second >=
+                      static_cast<int64_t>(S.g2fix) + 2 * static_cast<int64_t>(depth) + 1;
+        if (Cert && !proven) {
+          const int32_t oa = w == 0 ? s1 : s0, ob = w <= 1 ? s2 : s1, oc = w == 3 ? s2 : s3;
+          proven = certified_from_fixed(best, oa, ob, oc, depth, depth == cw, S.ln_pre, a.fast_qual, &q);
+        }
+        if (proven) {
+          c.depth = depth;
+          c.errors = depth - cw;
+          if (depth < a.min_reads) { c.base = 'N'; c.qual = 0; }
+          else if (q < a.min_cons_q) { c.base = 'N'; c.qual = 2; }
+          else { c.base = (0x54474341u >> (8u * w)) & 0xFFu; c.qual = q; }
+          done = true;
+        }
+      }
+    }
+    if (!done) {
+      c = exact_position<Src>(v, S, ref, n, pos, a.min_reads, a.min_cons_q, a.fast_qual);
+      ls.exact += c.depth >> 31;
+      c.depth &= ~kLiteralFlag;
+    }
+    ls.nocall += (c.base == 'N');
+    write_called(a, out_off + pos, c);
+  }
 }
 
 // Resolves a warp's queued positions.  The depth axis is split across a GROUP of lanes (8 lanes
@@ -717,83 +864,88 @@ __device__ __forceinline__ void slow_pass_g(const VoteArgs& a, const VoteSmem& S
       rb = un.read_begin; out_off = un.out_off;
       n = st.units[u + 1].read_begin - rb;
     }
-    const bool provable = n <= S.nmax2;
-    int32_t s0 = 0, s1 = 0, s2 = 0, s3 = 0;
-    uint32_t c01 = 0, c23 = 0;      // 4 x u16 observation counts; bit 31 of c23 = "unusable quality seen"
-    if (provable) {
-      for (uint32_t r = sub; r < n; r += G) {
-        uint64_t d = M::ld64(tv.reads + static_cast<typename M::off_t>(rb - tv.read_base + r) * 8u);
-        uint32_t len = static_cast<uint32_t>(d) & 0xFFFFu;
-        if (pos < len) {
-          typename M::off_t row = static_cast<typename M::off_t>((d >> 16) - tv.byte_base) + pos;
-          uint32_t b = M::ld8(tv.bases + row);
-          uint32_t q = M::ld8(tv.quals + row);
-          if (is_acgt_upper(b & 0xDFu)) {       // A,C,G,T in either case; 'N' and the rest are skipped
-            const uint32_t x = (b >> 1) & 3u;   // A 0, C 1, T 2, G 3
-            const uint32_t idx = x ^ (x >> 1);  // A 0, C 1, G 2, T 3
-            q = q > FGB_MAX_PHRED ? FGB_MAX_PHRED : q;
-            int32_t dq = S.dfix[q];
-            if (dq == INT32_MIN) { c23 |= 0x80000000u; dq = 0; }
-            s0 += idx == 0 ? dq : 0; s1 += idx == 1 ? dq : 0;
-            s2 += idx == 2 ? dq : 0; s3 += idx == 3 ? dq : 0;
-            c01 += idx == 0 ? 1u : (idx == 1 ? 0x10000u : 0u);
-            c23 += idx == 2 ? 1u : (idx == 3 ? 0x10000u : 0u);
-          }
-        }
-      }
+    resolve_group<StageObs<M>, G, Cert>(a, S, tv, valid, rb, n, pos, out_off, sub, ls);
+  }
+}
+
+// General kernel, shared-memory tiles: copies the pileups of the first kPileSlots queued positions out of the stage
+// into this warp's slots, so that the stage can be released before they are resolved (resolve_piles).  Returns the
+// number of slots filled, or 0 -- nothing to resolve from the slots, the whole queue is resolved in the stage -- when
+// one of these positions belongs to a unit deeper than a slot (a deep tile of an unsorted batch, a hand-made tile).
+template <bool Regular>
+__device__ __forceinline__ uint32_t gather_piles(const Stage& st, const TileView<ShMem>& tv, const uint32_t* wqueue,
+                                                 uint32_t qn, uint8_t* pile, uint32_t lane) {
+  const uint32_t np = qn < kPileSlots ? qn : kPileSlots;
+  bool deep = false;
+  // eight lanes per slot; lane `sub` copies reads sub, sub + 8, sub + 16 and places each covering one by its rank
+  // among the unit's covering reads
+  const uint32_t sub = lane & 7u, gshift = lane & ~7u;
+  const uint32_t uni_m = st.tile.flags >> 8;
+  const uint32_t reg_row0 = (st.tile.flags & kTileFlagSkew8) ? 8u : 0u;
+  for (uint32_t p0 = 0; p0 < np; p0 += 4u) {
+    const uint32_t p = p0 + (lane >> 3);
+    uint8_t* const slot = pile + p * kPileSlotBytes;
+    uint32_t pos = 0, rb = 0, n = 0;
+    uint64_t o = 0;
+    if (p < np) {
+      const uint32_t ent = wqueue[p];
+      const uint32_t u = ent >> 16;
+      pos = ent & 0xFFFFu;
+      const fgb_unit un = st.units[u];
+      rb = un.read_begin; o = un.out_off + pos;
+      n = st.units[u + 1].read_begin - rb;
     }
-    // butterfly over the group (n <= nmax2 <= 1024 keeps every 16-bit count and the flag intact)
+    deep |= __any_sync(0xFFFFFFFFu, n > kPileMaxObs);         // (reads past kPileMaxObs are never copied)
+    uint32_t b[3], q[3];
+    bool cov[3];
 #pragma unroll
-    for (uint32_t off = G >> 1; off > 0; off >>= 1) {
-      s0 += __shfl_xor_sync(0xFFFFFFFFu, s0, off);
-      s1 += __shfl_xor_sync(0xFFFFFFFFu, s1, off);
-      s2 += __shfl_xor_sync(0xFFFFFFFFu, s2, off);
-      s3 += __shfl_xor_sync(0xFFFFFFFFu, s3, off);
-      c01 += __shfl_xor_sync(0xFFFFFFFFu, c01, off);
-      uint32_t o23 = __shfl_xor_sync(0xFFFFFFFFu, c23, off);
-      c23 = ((c23 & 0x7FFFFFFFu) + (o23 & 0x7FFFFFFFu)) | ((c23 | o23) & 0x80000000u);
-    }
-    if (valid && sub == 0) {
-      Called c;
-      bool done = false;
-      if (provable) {
-        const uint32_t c0 = c01 & 0xFFFFu, c1 = c01 >> 16, c2 = c23 & 0xFFFFu, c3 = (c23 >> 16) & 0x7FFFu;
-        const uint32_t depth = c0 + c1 + c2 + c3;
-        if (depth == 0) {   // base_builder.rs:392-394 then vanilla_caller.rs:1345 (min_reads >= 1)
-          c.base = 'N'; c.qual = 0; c.depth = 0; c.errors = 0;
-          done = true;
-        } else if (!(c23 & 0x80000000u)) {
-          int32_t best = s0, second = INT32_MIN;
-          uint32_t w = 0, cw = c0;
-          if (s1 > best) { second = best; best = s1; w = 1; cw = c1; } else if (s1 > second) second = s1;
-          if (s2 > best) { second = best; best = s2; w = 2; cw = c2; } else if (s2 > second) second = s2;
-          if (s3 > best) { second = best; best = s3; w = 3; cw = c3; } else if (s3 > second) second = s3;
-          // every fixed-point term is within half a unit of D[q]*65536; two sums of <= depth terms
-          uint32_t q = a.fast_qual;
-          bool proven = static_cast<int64_t>(best) - second >=
-                        static_cast<int64_t>(S.g2fix) + 2 * static_cast<int64_t>(depth) + 1;
-          if (Cert && !proven) {
-            const int32_t oa = w == 0 ? s1 : s0, ob = w <= 1 ? s2 : s1, oc = w == 3 ? s2 : s3;
-            proven = certified_from_fixed(best, oa, ob, oc, depth, depth == cw, S.ln_pre, a.fast_qual, &q);
-          }
-          if (proven) {
-            c.depth = depth;
-            c.errors = depth - cw;
-            if (depth < a.min_reads) { c.base = 'N'; c.qual = 0; }
-            else if (q < a.min_cons_q) { c.base = 'N'; c.qual = 2; }
-            else { c.base = (0x54474341u >> (8u * w)) & 0xFFu; c.qual = q; }
-            done = true;
-          }
-        }
+    for (uint32_t j = 0; j < 3u; ++j) {
+      const uint32_t r = sub + 8u * j;
+      uint32_t row = 0;
+      if (Regular) {                                          // every read covers every position of its unit
+        cov[j] = r < n;
+        row = reg_row0 + (rb - st.tile.read_begin + r) * uni_m * 8u + pos;
+      } else {
+        cov[j] = r < n && StageObs<ShMem>::at(tv, rb, pos, r, row);
       }
-      if (!done) {
-        c = exact_position<M>(tv, S, rb, n, pos, a.min_reads, a.min_cons_q, a.fast_qual);
-        ls.exact += c.depth >> 31;
-        c.depth &= ~kLiteralFlag;
-      }
-      ls.nocall += (c.base == 'N');
-      write_called(a, out_off + pos, c);
+      b[j] = cov[j] ? tv.bases[row] : 0u;
+      q[j] = cov[j] ? tv.quals[row] : 0u;
     }
+    uint32_t before = 0;
+#pragma unroll
+    for (uint32_t j = 0; j < 3u; ++j) {
+      const uint32_t m = (__ballot_sync(0xFFFFFFFFu, cov[j]) >> gshift) & 0xFFu;
+      if (cov[j]) {
+        const uint32_t k = before + __popc(m & ((1u << sub) - 1u));
+        slot[kPileBases + k] = static_cast<uint8_t>(b[j]);
+        slot[kPileQuals + k] = static_cast<uint8_t>(q[j]);
+      }
+      before += __popc(m);
+    }
+    if (p < np && sub == 0u) {
+      *reinterpret_cast<uint64_t*>(slot) = o;
+      *reinterpret_cast<uint32_t*>(slot + 8u) = before | (n << 16);
+    }
+  }
+  return deep ? 0u : np;
+}
+
+// Resolves the slots gather_piles filled, four per pass, with the same group-of-8 proof and literal fallback as the
+// stage resolver.
+__device__ __forceinline__ void resolve_piles(const VoteArgs& a, const VoteSmem& S, const uint8_t* pile, uint32_t np,
+                                              uint32_t lane, LocalStats& ls) {
+  for (uint32_t p0 = 0; p0 < np; p0 += 4u) {
+    const uint32_t p = p0 + (lane >> 3);
+    const bool valid = p < np;
+    const uint8_t* const slot = pile + p * kPileSlotBytes;
+    uint32_t n_obs = 0, n = 0;
+    uint64_t o = 0;
+    if (valid) {
+      o = *reinterpret_cast<const uint64_t*>(slot);
+      const uint32_t m = *reinterpret_cast<const uint32_t*>(slot + 8u);
+      n_obs = m & 0xFFFFu; n = m >> 16;
+    }
+    resolve_group<PileObs, 8u, false>(a, S, slot, valid, n_obs, n, 0u, o, lane & 7u, ls);
   }
 }
 
@@ -848,10 +1000,14 @@ __device__ __forceinline__ void slow_pass(const VoteArgs& a, const VoteSmem& S, 
 // two-read units take the pair table in line.  (A sum-of-qualities proof for three- and four-read units was
 // built and measured: the exact threshold -- host_tables.cpp sumt -- has to guard against one very low
 // quality among high ones and ends up above what the per-read minimum test already accepts; dropped.)
-template <class M, bool Regular, int V = 0>
+//
+// Release (general kernel, shared-memory tiles): the warp copies the pileups its slow pass needs out of the stage
+// (gather_piles), releases stage s and only then resolves them, while the producer refills the stage.  Without it
+// the caller releases the stage after the tile.
+template <class M, bool Regular, int V = 0, bool Release = false>
 __device__ __forceinline__ void vote_tile(const VoteArgs& a, VoteSmem& S, const Stage& st,
                                           const TileView<M>& tv, uint32_t vt, uint32_t warp,
-                                          uint32_t n_items, LocalStats& ls) {
+                                          uint32_t n_items, LocalStats& ls, int s = 0) {
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t n_units = st.tile.n_units;
   const uint64_t out0 = st.units[0].out_off;
@@ -1164,9 +1320,18 @@ __device__ __forceinline__ void vote_tile(const VoteArgs& a, VoteSmem& S, const 
   //  the warp + __syncwarp() orders the byte stores below after it)
   uint32_t qn = *wcount;
   qn = qn < kWarpQueueCap ? qn : kWarpQueueCap;
-  if (qn) slow_pass<M, V == 1>(a, S, st, tv, wqueue, qn, lane, ls);
-  __syncwarp();
-  if (lane == 0) *wcount = 0;
+  if constexpr (Release) {
+    uint8_t* const pile = reinterpret_cast<uint8_t*>(&S) + sizeof(VoteSmem) + warp * (kPileSlots * kPileSlotBytes);
+    const uint32_t np = qn ? gather_piles<Regular>(st, tv, wqueue, qn, pile, lane) : 0u;
+    if (qn > np) slow_pass<M, false>(a, S, st, tv, wqueue + np, qn - np, lane, ls);   // what the slots did not take
+    __syncwarp();
+    if (lane == 0) { *wcount = 0; release_stage(S, s); }
+    if (np) resolve_piles(a, S, pile, np, lane, ls);
+  } else {
+    if (qn) slow_pass<M, V == 1>(a, S, st, tv, wqueue, qn, lane, ls);
+    __syncwarp();
+    if (lane == 0) *wcount = 0;
+  }
 }
 
 
@@ -1716,6 +1881,9 @@ __device__ __forceinline__ void vote_kernel_body(const Args& a) {
     }
     fence_mbar_init();
   }
+#if FGB_PIPE_TRACE
+  if (tid < kStages) { g_trace_arr_first[tid] = ~0ull; g_trace_arr_last[tid] = 0ull; g_trace_arr_n[tid] = 0u; }
+#endif
   __syncthreads();
 
   const uint32_t grid = gridDim.x;
@@ -1808,10 +1976,12 @@ __device__ __forceinline__ void vote_kernel_body(const Args& a) {
     ++tr_tiles;
     if (!landed) { ++tr_late; tr_lat += tv0 - *reinterpret_cast<const long long*>(&st.aux[2]); }
     if ((tid & 31u) == 0) g_trace_mark[warp] = -1;
+    if (tid == 0) g_trace_full0[s] = tv0;
 #endif
     // rotating item assignment: the partial last round of a tile lands on different warps from
     // tile to tile, so every warp does the same work in the long run
     const uint32_t vt = (tid - rot) & (kVoteThreads - 1);
+    bool released = false;                                     // the tile function released stage s
     uint32_t n_items = st.aux[1];
     if (n_items == 0)
       n_items = static_cast<uint32_t>((st.units[st.tile.n_units].out_off - st.units[0].out_off) >> 3);
@@ -1846,8 +2016,11 @@ __device__ __forceinline__ void vote_kernel_body(const Args& a) {
         } else if (st.tile.flags & kTileFlagRegular) vote_tile_deep<ShMem, true>(a, S, st, tv, tid, warp, n_items, ls);
         else vote_tile_deep<ShMem, false>(a, S, st, tv, tid, warp, n_items, ls);
       } else {
-        if (st.tile.flags & kTileFlagRegular) vote_tile<ShMem, true, V>(a, S, st, tv, vt, warp, n_items, ls);
-        else vote_tile<ShMem, false, V>(a, S, st, tv, vt, warp, n_items, ls);
+        // the general kernel releases the stage inside the tile; the duplex epilogue still reads it after the vote
+        constexpr bool kRelease = V == 0 && !Fused;
+        if (st.tile.flags & kTileFlagRegular) vote_tile<ShMem, true, V, kRelease>(a, S, st, tv, vt, warp, n_items, ls, s);
+        else vote_tile<ShMem, false, V, kRelease>(a, S, st, tv, vt, warp, n_items, ls, s);
+        released = kRelease;
       }
       if constexpr (Fused) {
         const uint2 tj = __ldg(reinterpret_cast<const uint2*>(a.tile_jobs + t));   // {begin, count | max_items << 16}
@@ -1867,7 +2040,7 @@ __device__ __forceinline__ void vote_kernel_body(const Args& a) {
       if (mark >= tv0) { tr_fast += mark - tv0; tr_slow += tv1 - mark; }
     }
 #endif
-    if ((tid & 31u) == 0) mbar_arrive(&S.empty[s]);   // this warp is done with stage s
+    if ((tid & 31u) == 0 && !released) release_stage(S, s);
   }
 #if FGB_PIPE_TRACE
   if ((tid & 31u) == 0) {

@@ -7,7 +7,9 @@ its byte mix.
 Diagnostic libraries (fgumi_b200/build.py build_variant, never the in-tree one):
   variants/pipe_trace.so   FGB_PIPE_TRACE=1: clock64 sums per CTA -- producer cycles waiting on `empty`, consumer-warp
                            cycles waiting on `full`, issue -> `full` cycles of the tiles that had not landed when the
-                           consumers arrived, voting cycles (fast pass / slow pass).  Loaded through FGUMI_B200_LIB.
+                           consumers arrived, voting cycles (fast pass / slow pass), how long a stage is held (warp 0
+                           passing `full` -> the last warp's release) and the spread of the eight warps' releases.
+                           Loaded through FGUMI_B200_LIB.
   variants/pipe_novote.so  FGB_PIPE_NOVOTE=1: consumers store constant words for their items instead of voting; the
                            producer, the stage ring, the prefetch and the stores are unchanged.
 
@@ -17,7 +19,8 @@ traced build's ms per launch beside the in-tree library's (the trace's own pertu
 the kernel's time, and -- for config 2 -- two ceilings on the bench's own device columns: a read-only torch pass, a
 two-read one-write torch pass (bases XOR quals as int64 into a third buffer: 67 % reads, the kernel moves 71 %), and
 the no-vote library.  `--compare` libraries (e.g. an A/B build, or another commit's library) are timed on the same
-batch, alternating with the in-tree one round by round, and their outputs are compared with its outputs.
+batch, alternating with the in-tree one round by round, and their outputs are compared with its outputs; the split of
+a traced --compare library (another commit's pipe_trace.so) is printed beside the in-tree sources' one.
 """
 from __future__ import annotations
 
@@ -85,6 +88,29 @@ class Lib:
         self.so.fgb_destroy(self.h)
 
 
+def split(tr, t_ms, launches):
+    """Fractions of the kernel's time from one traced round's counters (vote_kernel.cuh g_pipe_trace)."""
+    cta, ctas, warp_cyc, tiles = tr[0], tr[10], tr[2], tr[9]
+    clk_mhz = warp_cyc / (ctas * 8) / (t_ms * 1e-3) / 1e6     # ctas counts every launch's CTAs
+    period = (warp_cyc / (ctas * 8)) / (tiles / ctas) if tiles else None     # cycles per tile per CTA
+    return {
+        "ctas": ctas / launches,
+        "implied_sm_mhz": clk_mhz,
+        "producer_wait_empty_frac": tr[1] / cta if cta else None,
+        "consumer_wait_full_frac": tr[3] / warp_cyc,
+        "consumer_vote_frac": tr[4] / warp_cyc,
+        "consumer_fast_pass_frac": tr[5] / warp_cyc,
+        "consumer_slow_pass_frac": tr[6] / warp_cyc,
+        "consumer_other_frac": 1.0 - (tr[3] + tr[4]) / warp_cyc,
+        "tiles_not_landed_on_arrival_frac": tr[7] / tiles if tiles else None,
+        "issue_to_full_us_of_those": (tr[8] / tr[7]) / clk_mhz if tr[7] else None,
+        "tile_period_us": period / clk_mhz if tiles else None,
+        # warp 0 passing `full` -> the last warp's release of the stage, and last minus first release, per tile
+        "stage_hold_us": tr[11] / tiles / clk_mhz if tiles else None,
+        "release_skew_us": tr[12] / tiles / clk_mhz if tiles else None,
+    }
+
+
 def run(args):
     sys.path.insert(0, ROOT)
     import numpy as np
@@ -137,6 +163,7 @@ def run(args):
         time_launches(intree, plans[intree.name][1], cs, 1)
         ref = [x.clone() for x in (out.base, out.qual, out.depth, out.errors)]
         ms = {lib.name: [] for lib in [intree, trace] + others}
+        trs = {}
         same = {}
         for r in range(args.rounds):
             for lib in [intree, trace] + others:
@@ -145,7 +172,7 @@ def run(args):
                 t = time_launches(lib, plans[lib.name][1], cs, args.launches)
                 ms[lib.name].append(float(np.median(t)))
                 if lib.trace:
-                    tr = lib.read_trace(np)
+                    trs[lib.name] = lib.read_trace(np)
                 ok = all(torch.equal(a, b) for a, b in zip(ref, (out.base, out.qual, out.depth, out.errors)))
                 same[lib.name] = same.get(lib.name, True) and ok
         del ref
@@ -153,24 +180,10 @@ def run(args):
                                 for k, v in ms.items()}
         res["outputs_equal_in_tree"] = same
         res["tb_s"] = {k: gbps_bytes / (float(np.median(v)) * 1e-3) / 1e12 for k, v in ms.items()}
-        # the stall split of the traced build's last round (args.launches launches)
-        n = args.launches
-        cta, ctas, warp_cyc = tr[0], tr[10], tr[2]
-        t_ms = ms[trace.name][-1]
-        clk_mhz = warp_cyc / (ctas * 8) / (t_ms * 1e-3) / 1e6     # ctas counts every launch's CTAs
-        res["trace"] = {
-            "ctas": ctas / n,
-            "implied_sm_mhz": clk_mhz,
-            "producer_wait_empty_frac": tr[1] / cta if cta else None,
-            "consumer_wait_full_frac": tr[3] / warp_cyc,
-            "consumer_vote_frac": tr[4] / warp_cyc,
-            "consumer_fast_pass_frac": tr[5] / warp_cyc,
-            "consumer_slow_pass_frac": tr[6] / warp_cyc,
-            "consumer_other_frac": 1.0 - (tr[3] + tr[4]) / warp_cyc,
-            "tiles_not_landed_on_arrival_frac": tr[7] / tr[9] if tr[9] else None,
-            "issue_to_full_us_of_those": (tr[8] / tr[7]) / clk_mhz if tr[7] else None,
-            "tile_period_us": (warp_cyc / (ctas * 8)) / (tr[9] / ctas) / clk_mhz if tr[9] else None,
-        }
+        # the stall split of each traced build's last round (args.launches launches): the in-tree sources' and any
+        # traced --compare library's
+        res["trace"] = split(trs[trace.name], ms[trace.name][-1], args.launches)
+        res["trace_compare"] = {k: split(v, ms[k][-1], args.launches) for k, v in trs.items() if k != trace.name}
         if name == "config2":
             # data movement alone: the no-vote build on the same tiles (outputs are constants, not compared)
             nv = [float(np.median(time_launches(novote, plans[novote.name][1], cs, args.launches)))
