@@ -1478,7 +1478,10 @@ __device__ __forceinline__ void vote_tile_deep(const VoteArgs& a, VoteSmem& S, c
         }
       }
     }
-    // fold the group (every lane of the warp takes part; groups are aligned runs of g lanes)
+    // fold the group (every lane of the warp takes part; groups are aligned runs of g lanes).  The groups of one warp
+    // may hold units on both sides of an end of qt3 (nmax2, 255), so near_ok is not warp-uniform: the dissent
+    // counters are folded whenever any group needs them, since every lane must reach a full-mask shuffle.
+    const bool fold_near = __any_sync(0xFFFFFFFFu, near_ok);
     for (uint32_t off = g >> 1; off > 0; off >>= 1) {
       diff_lo |= __shfl_xor_sync(0xFFFFFFFFu, diff_lo, off);
       diff_hi |= __shfl_xor_sync(0xFFFFFFFFu, diff_hi, off);
@@ -1486,7 +1489,7 @@ __device__ __forceinline__ void vote_tile_deep(const VoteArgs& a, VoteSmem& S, c
       okq_hi &= __shfl_xor_sync(0xFFFFFFFFu, okq_hi, off);
       const uint32_t ml = __shfl_xor_sync(0xFFFFFFFFu, minlen, off);
       minlen = ml < minlen ? ml : minlen;
-      if (near_ok) {                                        // warp-uniform per group; byte counters stay below 256 (n < 255)
+      if (fold_near) {                                      // byte counters stay below 256 where used (n < 255)
         cnt_lo += __shfl_xor_sync(0xFFFFFFFFu, cnt_lo, off);
         cnt_hi += __shfl_xor_sync(0xFFFFFFFFu, cnt_hi, off);
         bad_lo |= __shfl_xor_sync(0xFFFFFFFFu, bad_lo, off);
