@@ -70,11 +70,8 @@ struct CodecMolecule {               // CODEC: one MI group that reached the vot
 };
 
 struct Prepared {
-  bool ok = false;
-  size_t surviving = 0;
   size_t n = 0;                    // live elements of `srs`; the rest is a pool whose buffers are reused
   std::vector<SourceRead> srs;
-  std::vector<uint32_t> rec_idx;   // indices (into the group's records) of the surviving reads
 };
 
 // The host threads of one caller, started once: fgb_caller_add_groups and the record assembly of a flush
@@ -141,7 +138,7 @@ class WorkerPool {
 };
 
 
-// ---- direct path (callers with a device) -----------------------------------------------------------
+// ---- direct path (simplex callers) ---------------------------------------------------------------------
 // The records of a batch are copied once into page-locked staging memory and shipped as they are
 // (FGB_IN_RECORDS); the host keeps only the per-read decisions (survival, row length, strand) and small
 // references into the staging copy (UMI, cell barcode, RX values).  Each context -- the caller itself
@@ -183,17 +180,21 @@ struct DSeg {                        // units [u0, u1) / reads [r0, r1) of one c
 struct PinBuf {                      // grow-only page-locked buffer
   void* p = nullptr;
   size_t cap = 0;
+  bool pageable = false;             // the owner has no device (FGB_DEVICE_NONE): ordinary heap memory, fgb_host_alloc needs a GPU
   fgb_status ensure(size_t bytes, size_t keep = 0) {
     if (bytes <= cap) return FGB_OK;
     const size_t ncap = bytes + bytes / 2 + 4096;
-    void* np = nullptr;
-    if (fgb_host_alloc(&np, ncap) != FGB_OK) return FGB_ERR_NOMEM;
+    void* np = pageable ? std::malloc(ncap) : nullptr;
+    if (pageable ? np == nullptr : fgb_host_alloc(&np, ncap) != FGB_OK) return FGB_ERR_NOMEM;
     if (keep) std::memcpy(np, p, keep);
-    fgb_host_free(p);
+    release();
     p = np; cap = ncap;
     return FGB_OK;
   }
-  void release() { fgb_host_free(p); p = nullptr; cap = 0; }
+  void release() {
+    if (pageable) std::free(p); else fgb_host_free(p);
+    p = nullptr; cap = 0;
+  }
 };
 
 }  // namespace
@@ -208,7 +209,7 @@ struct fgb_caller {
   UmiBuilder umi_builder;
   PrepOptions prep_opt;
   uint64_t stats[FGB_NSTATS] = {0};
-  Packer pack;
+  mutable Packer pack;                   // duplex / CODEC: the queued batch; planning-only simplex: what fgb_caller_pending laid out
   std::vector<Molecule> molecules;       // duplex
   std::vector<fgb_duplex_job> jobs;      // duplex
   uint64_t n_duplex_out = 0;
@@ -218,14 +219,14 @@ struct fgb_caller {
   uint64_t consensus_counter = 0;        // codec_caller.rs:1236
   std::vector<uint8_t> out;              // output of the last flush
   uint64_t out_count = 0;
-  std::string last_error;
+  mutable std::string last_error;        // (fgb_caller_pending, const, reports through it too)
   std::vector<uint32_t> ops;             // scratch
-  Prepared prepared[3];                  // simplex: fragment / R1 / R2 sub-groups, buffers reused across groups
-  std::vector<uint32_t> scratch_idx[6];  // simplex: kept / fragment / R1 / R2 record indices, [4] / [5] the alignment filter's before / after (track_rejects)
+  Prepared prepared[2];                  // simplex: [0] the alignment filter's pool; duplex: the X / Y pools; buffers reused across groups
+  std::vector<uint32_t> scratch_idx[5];  // simplex: kept / fragment / R1 / R2 record indices, [4] the alignment filter's survivors (track_rejects)
   overlap::Caller overlap{overlap::kAgreeConsensus, overlap::kDisagreeConsensus};   // simplex.rs:384-387
   std::vector<uint8_t> group_copy;       // mutable copy of a group for the overlap pre-pass
   std::vector<std::unique_ptr<fgb_caller>> workers;   // per-thread prep state of fgb_caller_add_groups (no GPU handle)
-  std::unique_ptr<WorkerPool> pool;                    // the threads themselves, started on first use
+  mutable std::unique_ptr<WorkerPool> pool;            // the threads themselves, started on first use
   // flush scratch that outlives a flush, so steady-state flushes neither page-fault nor zero-fill:
   uint8_t* joined = nullptr;                 // output stream of a flush (page-locked, grow-only)
   size_t joined_cap = 0, joined_len = 0;
@@ -233,13 +234,12 @@ struct fgb_caller {
   void* pinned[4] = {nullptr, nullptr, nullptr, nullptr};   // consensus columns, page-locked (fgb_host_alloc)
   size_t pinned_cap = 0;                     // capacity in elements (same for the four columns)
   // ---- direct path (see DirectPlan) ----
-  bool direct = false;                       // device caller, simplex: stage the records, build rows on the device
   DirectPlan dplan;                          // what THIS context queued (the caller itself or a worker)
   std::vector<DSeg> segs;                    // parent: ranges of the plans in input order
   PinBuf stage;                              // parent: the staged records
   size_t stage_len = 0;
   const uint8_t* zc_base = nullptr;          // parent: zero-copy batch (options.zero_copy_records): the caller's own page-locked blob
-  PinBuf d_reads, d_raws, d_units;           // parent: descriptor arrays handed to the engine
+  mutable PinBuf d_reads, d_raws, d_units;   // parent: descriptor arrays handed to the engine (fgb_caller_pending lays them out too)
   PinBuf px[12];                             // duplex / CODEC: page-locked result columns of a flush (grow-only)
   std::vector<View> views;                   // scratch: the records of the group being planned
   std::vector<uint64_t> rel_off;             // scratch: record offsets relative to the group
@@ -264,7 +264,7 @@ bool ensure_joined(fgb_caller* c, size_t total) {
 }
 
 // fn(0..T-1) on the caller's pool (T <= options.n_threads).
-void run_parallel(fgb_caller* c, uint32_t T, const std::function<void(uint32_t)>& fn) {
+void run_parallel(const fgb_caller* c, uint32_t T, const std::function<void(uint32_t)>& fn) {
   if (T <= 1) { if (T) fn(0); return; }
   if (!c->pool || c->pool->size() < T) c->pool.reset(new WorkerPool(std::max<uint32_t>(T, c->opt.n_threads)));
   if (!c->pool->run(T, fn)) throw std::bad_alloc();   // re-raised on the calling thread once every task has finished;
@@ -283,9 +283,9 @@ bool get_string_tag(const View& v, const char tag[2], std::string* out) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// simplex
+// simplex: the group rules on record headers only (no read is decoded here; the device -- or
+// fgb_caller_pending of a planning-only caller -- builds the SourceRead rows from the staged records)
 // ------------------------------------------------------------------------------------------------
-// process_subgroup up to the vote, vanilla_caller.rs:1124-1227
 // vanilla_caller.rs:752-754, 1061-1063, ...: the raw bytes of a rejected read, kept as a BAM record (block_size first).
 inline void keep_reject(fgb_caller* c, const View& v) {
   if (!c->opt.track_rejects) return;
@@ -297,124 +297,6 @@ inline void keep_reject(fgb_caller* c, const View& v) {
   ++c->reject_count;
 }
 
-void prepare_subgroup(fgb_caller* c, const std::vector<View>& recs, const std::vector<uint32_t>& members,
-                      Prepared* p) {
-  p->ok = false; p->surviving = 0; p->n = 0; p->rec_idx.clear();
-  const size_t min_reads = c->opt.min_reads;
-  if (members.empty()) return;
-  const bool track = c->opt.track_rejects != 0;
-  if (members.size() < min_reads) {
-    reject(c, FGB_STAT_REJ_INSUFFICIENT_READS, members.size());
-    if (track) for (uint32_t m : members) keep_reject(c, recs[m]);                     // :1137-1142
-    return;
-  }
-  size_t zero = 0;
-  for (uint32_t k = 0; k < members.size(); ++k) {
-    const View& v = recs[members[k]];
-    bam::cigar_ops(v, &c->ops);
-    size_t clip = bam::num_bases_extending_past_mate(v, c->ops);
-    if (p->n == p->srs.size()) p->srs.emplace_back();
-    if (make_source_read(c->prep_opt, v, k, clip, &c->ops, &p->srs[p->n])) ++p->n;
-    else { ++zero; keep_reject(c, v); }                                                // :1170-1174
-  }
-  if (zero) reject(c, FGB_STAT_REJ_ZERO_LENGTH, zero);
-  if (p->n < min_reads) {
-    if (p->n) {
-      reject(c, FGB_STAT_REJ_INSUFFICIENT_READS, p->n);
-      if (track) for (size_t i = 0; i < p->n; ++i) keep_reject(c, recs[members[p->srs[i].original_idx]]);   // :1180-1184
-    }
-    return;
-  }
-  std::vector<uint32_t>& before = c->scratch_idx[4];
-  if (track) { before.clear(); for (size_t i = 0; i < p->n; ++i) before.push_back(p->srs[i].original_idx); }
-  const size_t kept = filter_by_alignment_n(&p->srs, p->n);
-  if (kept != p->n) {
-    reject(c, FGB_STAT_REJ_MINORITY_ALIGNMENT, p->n - kept);
-    if (track) {                                                                       // :1193-1197, ascending
-      std::vector<uint32_t>& alive = c->scratch_idx[5];
-      alive.clear();
-      for (size_t i = 0; i < kept; ++i) alive.push_back(p->srs[i].original_idx);
-      std::sort(alive.begin(), alive.end());
-      std::sort(before.begin(), before.end());
-      for (uint32_t k : before)
-        if (!std::binary_search(alive.begin(), alive.end(), k)) keep_reject(c, recs[members[k]]);
-    }
-  }
-  p->n = kept;
-  if (p->n < min_reads) {
-    if (p->n) {
-      reject(c, FGB_STAT_REJ_INSUFFICIENT_READS, p->n);
-      if (track) for (size_t i = 0; i < p->n; ++i) keep_reject(c, recs[members[p->srs[i].original_idx]]);   // :1205-1209
-    }
-    return;
-  }
-  p->ok = true;
-  p->surviving = p->n;
-  for (size_t i = 0; i < p->n; ++i) p->rec_idx.push_back(members[p->srs[i].original_idx]);
-}
-
-void pack_simplex_unit(fgb_caller* c, const Prepared& p) { c->pack.add_unit(p.srs, p.n, c->opt.min_reads); }
-
-// consensus_reads for one MI group (vanilla_caller.rs:1477-1499 + process_group :1042-1114).
-fgb_status add_group_simplex(fgb_caller* c, const std::vector<View>& recs) {
-  const uint32_t n_records = static_cast<uint32_t>(recs.size());
-  const uint8_t* uv; size_t un;
-  if (!bam::find_string_tag(recs[0], c->opt.tag, &uv, &un)) {   // vanilla_caller.rs:1493-1496
-    c->last_error = std::string("Missing UMI tag '") + c->opt.tag[0] + c->opt.tag[1] + "'";
-    return FGB_ERR_MISSING_TAG;
-  }
-  c->stats[FGB_STAT_TOTAL_READS] += n_records;
-  std::vector<uint32_t>&kept = c->scratch_idx[0], &frag = c->scratch_idx[1], &r1 = c->scratch_idx[2], &r2 = c->scratch_idx[3];
-  kept.clear(); frag.clear(); r1.clear(); r2.clear();
-  for (uint32_t i = 0; i < n_records; ++i) {
-    uint16_t f = recs[i].flags();
-    if (!(f & bam::kSecondary) && !(f & bam::kSupplementary)) kept.push_back(i);
-  }
-  if (kept.size() != n_records) {
-    reject(c, FGB_STAT_REJ_SECONDARY_SUPPLEMENTARY, n_records - kept.size());
-    if (c->opt.track_rejects)                                                          // filter_reads, :745-757
-      for (uint32_t i = 0; i < n_records; ++i)
-        if (recs[i].flags() & (bam::kSecondary | bam::kSupplementary)) keep_reject(c, recs[i]);
-  }
-  if (kept.empty()) return FGB_OK;
-  if (kept.size() < c->opt.min_reads) {
-    reject(c, FGB_STAT_REJ_INSUFFICIENT_READS, kept.size());
-    for (uint32_t i : kept) keep_reject(c, recs[i]);                                   // :1061-1063
-    return FGB_OK;
-  }
-  for (uint32_t i : kept) {   // subgroup_reads, vanilla_caller.rs:1018-1039
-    uint16_t f = recs[i].flags();
-    if (!(f & bam::kPaired)) frag.push_back(i);
-    else if (f & bam::kFirst) r1.push_back(i);
-    else if (f & bam::kLast) r2.push_back(i);
-  }
-  if (frag.size() > 0xFFFFu || r1.size() > 0xFFFFu || r2.size() > 0xFFFFu) {
-    c->last_error = "a sub-group (fragment / R1 / R2 reads of one MI) has more than 65535 reads";
-    return FGB_ERR_UNIT_TOO_LARGE;
-  }
-  Prepared &pf = c->prepared[0], &p1 = c->prepared[1], &p2 = c->prepared[2];   // pooled across groups
-  prepare_subgroup(c, recs, frag, &pf);
-  if (pf.ok) { pack_simplex_unit(c, pf); c->stats[FGB_STAT_CONSENSUS_READS] += 1; }
-  prepare_subgroup(c, recs, r1, &p1);
-  prepare_subgroup(c, recs, r2, &p2);
-  if (p1.ok && p2.ok) {   // orphan rule, vanilla_caller.rs:1089-1108
-    pack_simplex_unit(c, p1);
-    pack_simplex_unit(c, p2);
-    c->stats[FGB_STAT_CONSENSUS_READS] += 2;
-  } else if (p1.ok) {
-    reject(c, FGB_STAT_REJ_ORPHAN_CONSENSUS, p1.surviving);
-    for (uint32_t ri : p1.rec_idx) keep_reject(c, recs[ri]);                           // :1095-1099
-  } else if (p2.ok) {
-    reject(c, FGB_STAT_REJ_ORPHAN_CONSENSUS, p2.surviving);
-    for (uint32_t ri : p2.rec_idx) keep_reject(c, recs[ri]);                           // :1101-1105
-  }
-  return FGB_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
-// simplex, direct path: the group rules of add_group_simplex on record headers only (no read is decoded;
-// the device builds the SourceRead rows from the staged records)
-// ------------------------------------------------------------------------------------------------
 struct DRead {                       // one record of a sub-group that yields a source read
   uint32_t rec;                      // index into the group's records
   uint32_t final_len;
@@ -514,7 +396,7 @@ bool plan_subgroup(fgb_caller* c, const std::vector<View>& recs, const std::vect
     if (kept != n) {
       reject(c, FGB_STAT_REJ_MINORITY_ALIGNMENT, n - kept);
       if (track) {                                                                     // :1193-1197, ascending input order
-        std::vector<uint32_t>& alive = c->scratch_idx[5];
+        std::vector<uint32_t>& alive = c->scratch_idx[4];
         alive.assign(n, 0u);
         for (size_t i = 0; i < kept; ++i) alive[pool.srs[i].original_idx] = 1u;
         for (size_t i = 0; i < n; ++i) if (!alive[i]) keep_reject(c, recs[(*out)[i].rec]);
@@ -828,12 +710,30 @@ size_t write_simplex_record_at(const fgb_caller* c, uint8_t* dst, const DUnit& u
   return total;
 }
 
-fgb_status flush_simplex_direct(fgb_caller* c) {
-  PhaseTrace trace;
-  // ---- global layout: prefix sums over the segments ----
+// fn(i) for every segment i of the queued batch, on up to options.n_threads of the caller's threads.
+void for_segs(const fgb_caller* c, const std::function<void(size_t)>& fn) {
   const size_t NS = c->segs.size();
-  std::vector<uint64_t> ub(NS + 1, 0), rbase(NS + 1, 0), bb(NS + 1, 0), ob(NS + 1, 0);
-  uint32_t max_reads = 0;
+  const uint32_t T = std::max<uint32_t>(1u, std::min<uint32_t>(std::max<uint32_t>(c->opt.n_threads, 1u), static_cast<uint32_t>(NS)));
+  if (T <= 1) { for (size_t i = 0; i < NS; ++i) fn(i); return; }
+  run_parallel(c, T, [&](uint32_t t) { for (size_t i = t; i < NS; i += T) fn(i); });
+}
+
+// The queued plans laid out as one batch (the flush's, and fgb_caller_pending's on a planning-only caller): prefix sums
+// over the segments, then every segment's descriptors at their global places in d_reads / d_raws / d_units, the
+// sentinel unit and two zero row descriptors behind them.
+struct DLayout {
+  std::vector<uint64_t> ub, rbase, bb, ob;   // per segment (and one past the last): first unit, read, row byte, output element
+  uint64_t U = 0, R = 0, n_bytes = 0, n_out = 0;
+  uint32_t max_reads = 0;                    // reads of the deepest unit
+  uint64_t* reads = nullptr;
+  fgb_raw_read* raws = nullptr;
+  fgb_unit* units = nullptr;
+};
+
+fgb_status lay_out_direct(const fgb_caller* c, DLayout* L) {
+  const size_t NS = c->segs.size();
+  std::vector<uint64_t> &ub = L->ub, &rbase = L->rbase, &bb = L->bb, &ob = L->ob;
+  ub.assign(NS + 1, 0); rbase.assign(NS + 1, 0); bb.assign(NS + 1, 0); ob.assign(NS + 1, 0);
   for (size_t i = 0; i < NS; ++i) {
     const DSeg& sg = c->segs[i];
     ub[i + 1] = ub[i] + (sg.u1 - sg.u0);
@@ -841,21 +741,17 @@ fgb_status flush_simplex_direct(fgb_caller* c) {
     bb[i + 1] = bb[i] + sg.row_bytes;
     ob[i + 1] = ob[i] + sg.out_elems;
   }
-  const uint64_t U = ub[NS], R = rbase[NS], n_bytes = bb[NS], no = ob[NS];
+  const uint64_t U = ub[NS], R = rbase[NS];
+  L->U = U; L->R = R; L->n_bytes = bb[NS]; L->n_out = ob[NS];
   if (!U) return FGB_OK;
   if (U >= 0xFFFFFFFFull || R >= 0xFFFFFFFFull) { c->last_error = "batch too large"; return FGB_ERR_INVALID_ARG; }
   if (c->d_reads.ensure((R + 2) * sizeof(uint64_t)) != FGB_OK || c->d_raws.ensure((R + 1) * sizeof(fgb_raw_read)) != FGB_OK ||
       c->d_units.ensure((U + 1) * sizeof(fgb_unit)) != FGB_OK) { c->last_error = "out of page-locked memory"; return FGB_ERR_NOMEM; }
-  uint64_t* g_reads = static_cast<uint64_t*>(c->d_reads.p);
-  fgb_raw_read* g_raws = static_cast<fgb_raw_read*>(c->d_raws.p);
-  fgb_unit* g_units = static_cast<fgb_unit*>(c->d_units.p);
-  const uint32_t T = std::max<uint32_t>(1u, std::min<uint32_t>(std::max<uint32_t>(c->opt.n_threads, 1u), static_cast<uint32_t>(NS)));
+  uint64_t* g_reads = L->reads = static_cast<uint64_t*>(c->d_reads.p);
+  fgb_raw_read* g_raws = L->raws = static_cast<fgb_raw_read*>(c->d_raws.p);
+  fgb_unit* g_units = L->units = static_cast<fgb_unit*>(c->d_units.p);
   std::vector<uint32_t> seg_max(NS, 0);
-  auto for_segs = [&](const std::function<void(size_t)>& fn) {
-    if (T <= 1) { for (size_t i = 0; i < NS; ++i) fn(i); return; }
-    run_parallel(c, T, [&](uint32_t t) { for (size_t i = t; i < NS; i += T) fn(i); });
-  };
-  for_segs([&](size_t i) {       // descriptors of segment i at their global places
+  for_segs(c, [&](size_t i) {    // descriptors of segment i at their global places
     const DSeg& sg = c->segs[i];
     const DirectPlan& P = sg.ctx->dplan;
     uint64_t off = bb[i], oo = ob[i], r = rbase[i];
@@ -879,16 +775,31 @@ fgb_status flush_simplex_direct(fgb_caller* c) {
   });
   {
     fgb_unit sentinel;
-    sentinel.out_off = no; sentinel.read_begin = static_cast<uint32_t>(R); sentinel.cons_len = 0;
+    sentinel.out_off = L->n_out; sentinel.read_begin = static_cast<uint32_t>(R); sentinel.cons_len = 0;
     g_units[U] = sentinel;
     g_reads[R] = 0; g_reads[R + 1] = 0;
   }
-  for (uint32_t m : seg_max) max_reads = m > max_reads ? m : max_reads;
+  for (uint32_t m : seg_max) L->max_reads = m > L->max_reads ? m : L->max_reads;
+  return FGB_OK;
+}
+
+fgb_status flush_simplex_direct(fgb_caller* c) {
+  PhaseTrace trace;
+  DLayout L;
+  const fgb_status lst = lay_out_direct(c, &L);
+  if (lst != FGB_OK || !L.U) return lst;
+  const size_t NS = c->segs.size();
+  const std::vector<uint64_t> &ub = L.ub, &bb = L.bb;
+  const uint64_t U = L.U, R = L.R, n_bytes = L.n_bytes, no = L.n_out;
+  const uint32_t max_reads = L.max_reads;
+  uint64_t* const g_reads = L.reads;
+  fgb_raw_read* const g_raws = L.raws;
+  fgb_unit* const g_units = L.units;
   trace.mark("descriptors");
   // ---- tiles: every segment plans its own range (a tile never spans two segments) ----
   std::vector<std::vector<fgb_tile>> seg_tiles(NS);
   std::vector<fgb_status> seg_st(NS, FGB_OK);
-  for_segs([&](size_t i) {
+  for_segs(c, [&](size_t i) {
     uint64_t prev_end = bb[i];
     seg_tiles[i].clear();
     seg_st[i] = plan_tiles_range(g_units, ub[i], ub[i + 1], g_reads, R, &prev_end, [&](const fgb_tile& t) { seg_tiles[i].push_back(t); });
@@ -920,7 +831,7 @@ fgb_status flush_simplex_direct(fgb_caller* c) {
     std::memcpy(strs + c->prefix.size(), c->rg.data(), c->rg.size());
     const uint8_t* const stage0 = c->zc_base ? c->zc_base : static_cast<const uint8_t*>(c->stage.p);
     std::vector<int> bad(NS, 0);
-    for_segs([&](size_t i) {       // jobs and strings of segment i; the RX consensus (simple_umi.rs:236-245) is computed here
+    for_segs(c, [&](size_t i) {       // jobs and strings of segment i; the RX consensus (simple_umi.rs:236-245) is computed here
       const DSeg& sg = c->segs[i];
       const DirectPlan& P = sg.ctx->dplan;
       uint64_t ro = rb_[i], so_ = sb_[i];
@@ -2021,9 +1932,8 @@ static fgb_status caller_create_impl(int device, const fgb_caller_options* opt, 
   if (device != FGB_DEVICE_NONE) {       // FGB_DEVICE_NONE: planning only, flush refuses (no CPU fallback)
     fgb_status st = fgb_create(device, &p, &c->h);
     if (st != FGB_OK) return st;
-    // simplex callers with a device build the source-read rows on the device (planning-only callers decode them
-    // on the host, so the packed rows can be inspected)
-    c->direct = opt->mode == FGB_MODE_SIMPLEX;
+  } else {                               // what a planning-only simplex caller stages and lays out lives on the heap
+    for (PinBuf* b : {&c->stage, &c->d_reads, &c->d_raws, &c->d_units}) b->pageable = true;
   }
   *out = c.release();
   return FGB_OK;
@@ -2041,10 +1951,29 @@ fgb_status fgb_caller_take_rejects(fgb_caller* c, const uint8_t** data, uint64_t
   return FGB_OK;
 }
 
-fgb_status fgb_caller_pending(const fgb_caller* c, fgb_batch* batch, const fgb_duplex_job** duplex_jobs,
-                              uint64_t* n_duplex_jobs, const fgb_codec_job** codec_jobs,
-                              uint64_t* n_codec_jobs) {
+static fgb_status caller_pending_impl(const fgb_caller* c, fgb_batch* batch, const fgb_duplex_job** duplex_jobs,
+                                      uint64_t* n_duplex_jobs, const fgb_codec_job** codec_jobs,
+                                      uint64_t* n_codec_jobs) {
   if (!c || !batch) return FGB_ERR_INVALID_ARG;
+  if (c->opt.mode == FGB_MODE_SIMPLEX && !c->h) {
+    // planning only: the queued plans laid out as the flush lays them out, each row decoded from its staged record
+    // the way the device builds it (a caller with a device reports the empty Packer: its rows exist on the device only)
+    DLayout L;
+    const fgb_status st = lay_out_direct(c, &L);
+    if (st != FGB_OK) return st;
+    Packer& pk = c->pack;
+    pk.reads.assign(L.reads, L.reads + L.R);
+    pk.units.assign(L.units, L.units + L.U);
+    pk.n_out = L.n_out;
+    pk.bases.assign(L.n_bytes, 0);
+    pk.quals.assign(L.n_bytes, 0);
+    const uint8_t* const stage = static_cast<const uint8_t*>(c->stage.p);
+    for (uint64_t r = 0; r < L.R; ++r) {
+      const uint64_t off = FGB_READ_OFF(L.reads[r]);
+      decode_source_row(stage + L.raws[r].src_off, L.raws[r].raw_len, L.raws[r].flags & FGB_RAW_REVERSE, FGB_READ_LEN(L.reads[r]),
+                        c->prep_opt.min_input_base_quality, pk.bases.data() + off, pk.quals.data() + off);
+    }
+  }
   std::memset(batch, 0, sizeof(*batch));
   batch->n_units = c->pack.units.size();
   batch->n_reads = c->pack.reads.size();
@@ -2085,7 +2014,7 @@ static fgb_status caller_add_group_impl(fgb_caller* c, const uint8_t* records, c
                                 uint32_t n_records) {
   if (!c || (n_records && (!records || !rec_off))) return FGB_ERR_INVALID_ARG;
   if (n_records == 0) return FGB_OK;
-  if (c->direct) {
+  if (c->opt.mode == FGB_MODE_SIMPLEX) {
     const uint64_t grp[2] = {0, n_records};
     return direct_add(c, records, rec_off, grp, 1);
   }
@@ -2102,9 +2031,9 @@ static fgb_status caller_add_group_impl(fgb_caller* c, const uint8_t* records, c
       return FGB_ERR_UNIT_TOO_LARGE;
     }
   }
-  if (n_records > 0xFFFFu && c->opt.mode != FGB_MODE_SIMPLEX) {   // u16 observation counters (base_builder.rs:236): say so
+  if (n_records > 0xFFFFu) {                                        // u16 observation counters (base_builder.rs:236): say so
     c->last_error = "an MI group has more than 65535 reads";       // now, not at flush time with every other group queued
-    return FGB_ERR_UNIT_TOO_LARGE;                                  // (simplex checks its three sub-groups)
+    return FGB_ERR_UNIT_TOO_LARGE;
   }
   if (c->opt.consensus_call_overlapping_bases) {   // simplex.rs:395-398, duplex.rs:464-467
     const uint64_t base = rec_off[0], total = rec_off[n_records] - base;
@@ -2115,8 +2044,7 @@ static fgb_status caller_add_group_impl(fgb_caller* c, const uint8_t* records, c
     for (uint32_t i = 0; i < n_records; ++i) recs[i] = View(c->group_copy.data() + off[i], off[i + 1] - off[i]);
   }
   if (c->opt.mode == FGB_MODE_DUPLEX) return add_group_duplex(c, recs);
-  if (c->opt.mode == FGB_MODE_CODEC) return add_group_codec(c, recs);
-  return add_group_simplex(c, recs);
+  return add_group_codec(c, recs);
 }
 
 }  // extern "C"
@@ -2257,9 +2185,10 @@ void merge_workers_parallel(fgb_caller* c, uint32_t T) {
 
 namespace {
 
-// The direct path's add: stages the records of groups [0, n_groups) (one contiguous slice of the blob) in
-// page-locked memory and plans them, on options.n_threads threads over contiguous ranges of groups.  All or
-// nothing: on an error nothing of this call stays queued (the same for one thread and for many).
+// The simplex caller's add: stages the records of groups [0, n_groups) (one contiguous slice of the blob) in
+// page-locked memory (ordinary heap memory without a device) and plans them, on options.n_threads threads over
+// contiguous ranges of groups.  All or nothing: on an error nothing of this call stays queued (the same for one
+// thread and for many).
 fgb_status direct_add(fgb_caller* c, const uint8_t* records, const uint64_t* rec_off, const uint64_t* group_rec,
                       uint64_t n_groups) {
   const uint64_t rec0 = group_rec[0], rec1 = group_rec[n_groups];
@@ -2268,7 +2197,7 @@ fgb_status direct_add(fgb_caller* c, const uint8_t* records, const uint64_t* rec
   if (b1 < b0) { c->last_error = "record offsets must ascend"; return FGB_ERR_LAYOUT; }
   // zero-copy batches: the records are shipped from the caller's own page-locked blob (decided by the first add
   // of a batch); otherwise this call's slice of the blob is staged in page-locked memory owned by the caller object
-  if (c->opt.zero_copy_records && c->segs.empty() && c->stage_len == 0 && !c->zc_base && fgb_host_is_pinned(records) &&
+  if (c->h && c->opt.zero_copy_records && c->segs.empty() && c->stage_len == 0 && !c->zc_base && fgb_host_is_pinned(records) &&
       !(c->opt.consensus_call_overlapping_bases && (c->prep_opt.trim || c->opt.track_rejects)))   // those run the pre-pass on the host, in the staged copy
     c->zc_base = records;
   const bool zc = c->zc_base != nullptr;
@@ -2339,9 +2268,9 @@ fgb_status direct_add(fgb_caller* c, const uint8_t* records, const uint64_t* rec
         x->rel_off.resize(n + 1);
         for (uint32_t i = 0; i <= n; ++i) x->rel_off[i] = rec_off[r0 + i] - rec_off[r0];
         uint8_t* const gbase = stage + dst0 + (rec_off[r0] - b0);
-        // The device co-calls the overlaps on the uploaded records (the host only plans the runs) unless the
-        // quality trim needs whole rewritten reads or a mate has no qualities (0xFF): then in place, here.
-        bool on_device = !c->prep_opt.trim && !c->opt.track_rejects;   // (rejected reads are kept as the pre-pass leaves them: on the host then)
+        // The device co-calls the overlaps on the uploaded records (the host only plans the runs) unless there is no
+        // device, the quality trim needs whole rewritten reads or a mate has no qualities (0xFF): then in place, here.
+        bool on_device = c->h && !c->prep_opt.trim && !c->opt.track_rejects;   // (rejected reads are kept as the pre-pass leaves them: on the host then)
         if (on_device) {
           x->overlap.plan_group(gbase, x->rel_off.data(), n, &x->group_runs);
           for (const overlap::Run& r : x->group_runs) {
@@ -2435,7 +2364,7 @@ static fgb_status caller_add_groups_impl(fgb_caller* c, const uint8_t* records, 
                                  const uint64_t* group_rec, uint64_t n_groups) {
   if (!c || (n_groups && (!records || !rec_off || !group_rec))) return FGB_ERR_INVALID_ARG;
   if (n_groups == 0) return FGB_OK;
-  if (c->direct) return direct_add(c, records, rec_off, group_rec, n_groups);
+  if (c->opt.mode == FGB_MODE_SIMPLEX) return direct_add(c, records, rec_off, group_rec, n_groups);
   const uint64_t n_rec = group_rec[n_groups] - group_rec[0];
   uint32_t T = static_cast<uint32_t>(std::min<uint64_t>(std::max<uint32_t>(c->opt.n_threads, 1u), (n_groups + 63) / 64));
   auto run = [&](fgb_caller* dst, uint64_t g0, uint64_t g1, uint64_t* bad_group) -> fgb_status {
@@ -2502,13 +2431,11 @@ static fgb_status caller_flush_impl(fgb_caller* c, const uint8_t** out_data, uin
   fgb_status st = c->opt.mode == FGB_MODE_DUPLEX ? flush_duplex(c)
                   : c->opt.mode == FGB_MODE_CODEC ? flush_codec(c)
                   : flush_simplex_direct(c);
-  if (c->direct) {
-    c->dplan.clear();
-    for (auto& w : c->workers) w->dplan.clear();
-    c->segs.clear();
-    c->stage_len = 0;
-    c->zc_base = nullptr;
-  }
+  c->dplan.clear();
+  for (auto& w : c->workers) w->dplan.clear();
+  c->segs.clear();
+  c->stage_len = 0;
+  c->zc_base = nullptr;
   c->pack.clear(); c->molecules.clear(); c->jobs.clear();
   c->codec_molecules.clear(); c->codec_jobs.clear();
   c->n_duplex_out = 0; c->n_codec_out = 0;
@@ -2803,6 +2730,10 @@ fgb_status fgb_caller_add_groups(fgb_caller* c, const uint8_t* records, const ui
 }
 fgb_status fgb_caller_flush(fgb_caller* c, const uint8_t** out_data, uint64_t* out_len, uint64_t* out_count) {
   FGB_GUARD(c, caller_flush_impl(c, out_data, out_len, out_count))
+}
+fgb_status fgb_caller_pending(const fgb_caller* c, fgb_batch* batch, const fgb_duplex_job** duplex_jobs,
+                              uint64_t* n_duplex_jobs, const fgb_codec_job** codec_jobs, uint64_t* n_codec_jobs) {
+  FGB_GUARD(c, caller_pending_impl(c, batch, duplex_jobs, n_duplex_jobs, codec_jobs, n_codec_jobs))
 }
 
 }  // extern "C"

@@ -180,19 +180,13 @@ inline uint32_t plan_read_len(const PrepOptions& opt, const View& v, size_t mate
   return plan_read_len_eff(opt, v, mate_clip, [](size_t, uint8_t*, uint8_t*) {});
 }
 
-inline bool make_source_read(const PrepOptions& opt, const View& v, uint32_t idx, size_t mate_clip,
-                             std::vector<uint32_t>* ops, SourceRead* sr) {
-  const size_t bound = plan_read_len(opt, v, mate_clip);     // only these oriented positions survive
-  if (bound == 0) return false;
-  const bool neg = v.flags() & bam::kReverse;
-  const uint8_t min_bq = opt.min_input_base_quality;
-  const uint32_t read_len = v.l_seq();
-  const uint8_t* s = v.b + v.seq_off();
-  const uint8_t* q = v.b + v.qual_off();
-  sr->bases.resize(bound);
-  sr->quals.resize(bound);
-  uint8_t* __restrict ob = sr->bases.data();
-  uint8_t* __restrict oq = sr->quals.data();
+// The per-base half of create_source_read (vanilla_caller.rs:893-916): the first `bound` oriented positions of a read
+// whose packed sequence starts at `s` (read_len bases, the qualities (read_len + 1) / 2 bytes later), decoded,
+// reverse-complemented when `neg`, and (N, 2) where the quality is below min_bq -- the row the device builds from a
+// staged record (FGB_IN_RECORDS).
+inline void decode_source_row(const uint8_t* s, uint32_t read_len, bool neg, size_t bound, uint8_t min_bq,
+                              uint8_t* __restrict ob, uint8_t* __restrict oq) {
+  const uint8_t* q = s + (read_len + 1) / 2;
   // a pair table decodes one packed byte (two bases) per step, complemented and swapped for
   // negative-strand reads; then a (reversed) copy of the qualities and a compare-and-blend pass that
   // the compiler vectorises
@@ -225,6 +219,16 @@ inline bool make_source_read(const PrepOptions& opt, const View& v, uint32_t idx
     ob[i] = low ? static_cast<uint8_t>('N') : ob[i];
     oq[i] = low ? static_cast<uint8_t>(2) : oq[i];
   }
+}
+
+inline bool make_source_read(const PrepOptions& opt, const View& v, uint32_t idx, size_t mate_clip,
+                             std::vector<uint32_t>* ops, SourceRead* sr) {
+  const size_t bound = plan_read_len(opt, v, mate_clip);     // only these oriented positions survive
+  if (bound == 0) return false;
+  const bool neg = v.flags() & bam::kReverse;
+  sr->bases.resize(bound);
+  sr->quals.resize(bound);
+  decode_source_row(v.b + v.seq_off(), v.l_seq(), neg, bound, opt.min_input_base_quality, sr->bases.data(), sr->quals.data());
   const size_t final_len = bound;                            // the trailing Ns are already gone
   bam::cigar_ops(v, ops);
   bam::simplify_cigar(*ops, &sr->cigar);
@@ -340,10 +344,8 @@ struct Packer {
   std::vector<fgb_unit> units;
   uint64_t n_out = 0;
   // Appends one unit (its SourceRead rows); returns the unit index.
-  uint32_t add_unit(const std::vector<SourceRead>& srs, size_t min_reads) { return add_unit(srs, srs.size(), min_reads); }
-  // ... the first `n` elements of `srs`
-  uint32_t add_unit(const std::vector<SourceRead>& srs, size_t n, size_t min_reads) {
-    return add_unit_rows(n, min_reads, [&](size_t k) -> const SourceRead& { return srs[k]; });
+  uint32_t add_unit(const std::vector<SourceRead>& srs, size_t min_reads) {
+    return add_unit_rows(srs.size(), min_reads, [&](size_t k) -> const SourceRead& { return srs[k]; });
   }
   // ... rows given by pointer (the duplex caller splits one pooled vector into four sub-families)
   uint32_t add_unit(const std::vector<const SourceRead*>& rows, size_t min_reads) {

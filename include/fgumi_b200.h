@@ -771,14 +771,18 @@ fgb_status fgb_overlap_apply_group(uint8_t* records, const uint64_t* rec_off, ui
 typedef struct fgb_caller fgb_caller;
 /* device >= 0: a caller with its own engine handle on that GPU.
  * device == FGB_DEVICE_NONE: a PLANNING-ONLY caller -- fgb_caller_add_group(s) run the whole host prep
- * and queue the packed batch, fgb_caller_pending exposes it, and fgb_caller_flush fails with
- * FGB_ERR_NO_DEVICE.  It computes no consensus (there is no CPU fallback); it exists so the host side of
- * the three callers can be inspected and tested on a machine without a GPU. */
+ * and queue the batch, fgb_caller_pending exposes it, and fgb_caller_flush fails with FGB_ERR_NO_DEVICE.
+ * It makes no CUDA call and computes no consensus (there is no CPU fallback); it exists so the host side of
+ * the three callers can be inspected and tested on a machine without a GPU.  A simplex caller plans on
+ * record headers as a caller with a device does (the overlapping-bases pre-pass runs on the host, in its
+ * copy of the records); fgb_caller_pending lays the plans out as a flush would and decodes the rows from
+ * that copy. */
 #define FGB_DEVICE_NONE (-1)
 fgb_status fgb_caller_create(int device, const fgb_caller_options* opt, fgb_caller** out);
 /* What is queued for the next flush: the packed batch (tiles not planned yet: tiles = NULL, n_tiles = 0;
  * units[] holds n_units entries WITHOUT the sentinel, so the reads of the last unit end at n_reads), the
- * duplex jobs and the CODEC jobs.  Host pointers, valid until the next add / flush / destroy. */
+ * duplex jobs and the CODEC jobs.  Host pointers, valid until the next add / flush / destroy.  A simplex
+ * caller with a device builds its rows on the device and reports an empty batch here. */
 fgb_status fgb_caller_pending(const fgb_caller* c, fgb_batch* batch, const fgb_duplex_job** duplex_jobs,
                               uint64_t* n_duplex_jobs, const fgb_codec_job** codec_jobs,
                               uint64_t* n_codec_jobs);

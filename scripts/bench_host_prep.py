@@ -1,5 +1,7 @@
-"""Host-prep throughput of the record-level callers on the CPU alone (planning-only callers: group
-rules + source-read prep + packing, no vote): input reads per second of fgb_caller_add_groups."""
+"""Host-prep throughput of the record-level callers on the CPU alone (planning-only callers, no vote): input
+reads per second of fgb_caller_add_groups.  Simplex measures the product's simplex planning: the staging copy
+of the records plus the header-only group decisions (the rows are built on the device later); duplex and CODEC
+measure group rules + source-read decode + packing."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
