@@ -10,5 +10,6 @@ from .engine import (Engine, PackedBatch, HostColumns, DeviceBatch, DeviceColumn
                      TILE_JOBS_DTYPE, plan_tiles_jobs)
 from . import lib  # noqa: F401
 from .caller import VanillaUmiConsensusCaller, DuplexConsensusCaller, CodecConsensusCaller, ConsensusOutput, ConsensusFilter, DuplexConsensusFilter, apply_overlapping_consensus, bgzf_compress, write_bam  # noqa: F401
+from .umi import UmiAssigner, UmiAssignment  # noqa: F401
 
 __version__ = "0.1.0"

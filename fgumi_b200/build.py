@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libfgumi_b200.so")
-SOURCES = ["capi.cu", "host_tables.cpp", "host/caller_host.cpp", "host/bgzf.cpp"]
+SOURCES = ["capi.cu", "host_tables.cpp", "host/caller_host.cpp", "host/bgzf.cpp", "host/umi_host.cpp"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-maxrregcount=112",      # upper bound only; vote_kernel must land at <= 96 (see _check_vote_kernel)
@@ -41,6 +41,21 @@ def _check_vote_kernel(ptxas_log: str) -> None:
                          "spill stores; expected <= 96 and <= 16 (occupancy drops to one CTA per SM above 96)\n")
 
 
+def _check_umi_kernels(ptxas_log: str) -> None:
+    """The UMI edge kernels keep a query key and a short scalar state per thread in registers: a spill or a stack
+    frame means a source change pushed the comparator into local memory, and fails the build."""
+    import re
+    found = 0
+    for m in re.finditer(r"Function properties for (\S*umi_\w+_kernel\S*)\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores",
+                         ptxas_log):
+        found += 1
+        if int(m.group(2)) or int(m.group(3)):
+            raise RuntimeError(f"fgumi_b200 build: {m.group(1)} has a {m.group(2)}-byte stack frame and spills "
+                               f"{m.group(3)} bytes (expected none)")
+    if found != 4:
+        raise RuntimeError(f"fgumi_b200 build: ptxas reported {found} UMI edge kernels, expected 4")
+
+
 def build(force: bool = False, verbose: bool = False) -> str:
     deps = [os.path.join(dp, f) for dp, _, fs in os.walk(CSRC) for f in fs]
     deps.append(os.path.join(HERE, "..", "include", "fgumi_b200.h"))
@@ -54,6 +69,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if r.returncode != 0:
         raise RuntimeError("nvcc failed building libfgumi_b200.so")
     _check_vote_kernel(r.stdout + r.stderr)
+    _check_umi_kernels(r.stdout + r.stderr)
     return OUT
 
 

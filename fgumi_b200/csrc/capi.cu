@@ -21,7 +21,11 @@
 #include "inflate_kernel.cuh"
 #include "host_tables.h"
 #include "planner.h"
+#include "umi_kernels.cuh"
 #include "unpack_kernels.cuh"
+#include "host/umi_host.h"
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 #include "vote_kernel.cuh"
 
 using namespace fgb;
@@ -106,6 +110,19 @@ struct fgb_handle {
   std::vector<TraceMark> trace_ev;                  // device timeline of the last submit
   std::chrono::steady_clock::time_point trace_t0, trace_t1;
   uint8_t* d_dstatus = nullptr; uint64_t cap_dstatus = 0;   // fgb_vote_duplex_device: job status bytes when the caller wants none
+  struct UmiBufs {                                   // fgb_umi_assign: device buffers and their page-locked staging
+    fgb_umi_key* keys = nullptr; uint8_t* blob = nullptr; fgb::UmiWork* work = nullptr;
+    uint64_t* deg = nullptr; uint64_t* off = nullptr; uint32_t* edges = nullptr;
+    uint64_t* sbits_in = nullptr; uint64_t* sbits = nullptr; uint32_t* sidx_in = nullptr; uint32_t* sidx = nullptr;
+    uint8_t* temp = nullptr;
+    uint64_t cap_keys = 0, cap_blob = 0, cap_work = 0, cap_deg = 0, cap_off = 0, cap_edges = 0, cap_sbits_in = 0,
+             cap_sbits = 0, cap_sidx_in = 0, cap_sidx = 0, cap_temp = 0;
+    fgb_umi_key* h_keys = nullptr; uint8_t* h_blob = nullptr; fgb::UmiWork* h_work = nullptr;
+    uint64_t* h_sbits = nullptr; uint32_t* h_sidx = nullptr; uint64_t* h_off = nullptr; uint32_t* h_edges = nullptr;
+    uint64_t hcap_keys = 0, hcap_blob = 0, hcap_work = 0, hcap_sbits = 0, hcap_sidx = 0, hcap_off = 0, hcap_edges = 0;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;   // around the count and fill passes
+    double timing[4] = {0, 0, 0, 0};                 // fgb_umi_last_timing
+  } umi;
 };
 
 namespace {
@@ -333,6 +350,14 @@ void fgb_destroy(fgb_handle* h) {
   cudaFree(h->d_oruns);
   cudaFree(h->d_recstr); cudaFree(h->d_recjobs);
   cudaFree(h->d_dstatus);
+  {
+    auto& u = h->umi;
+    cudaFree(u.keys); cudaFree(u.blob); cudaFree(u.work); cudaFree(u.deg); cudaFree(u.off); cudaFree(u.edges);
+    cudaFree(u.sbits_in); cudaFree(u.sbits); cudaFree(u.sidx_in); cudaFree(u.sidx); cudaFree(u.temp);
+    cudaFreeHost(u.h_keys); cudaFreeHost(u.h_blob); cudaFreeHost(u.h_work); cudaFreeHost(u.h_sbits);
+    cudaFreeHost(u.h_sidx); cudaFreeHost(u.h_off); cudaFreeHost(u.h_edges);
+    for (cudaEvent_t ev : {u.ev0, u.ev1, u.ev2, u.ev3}) if (ev) cudaEventDestroy(ev);
+  }
   if (h->ev_recstr) cudaEventDestroy(h->ev_recstr);
   delete h;
 }
@@ -1320,5 +1345,324 @@ fgb_status fgb_stats_reset(fgb_handle* h) {
 
 uint64_t fgb_launch_count(const fgb_handle* h) { return h ? h->launches : 0; }
 uint32_t fgb_engine_caps(void) { return FGB_CAP_RECORD_ASSEMBLY; }
+
+}  // extern "C"
+
+// ---- UMI assignment (umi_kernels.cuh, host/umi_host.cpp) ----------------------------------------------------------
+namespace {
+
+template <class T>
+fgb_status ensure_pinned(fgb_handle* h, T** p, uint64_t* cap, uint64_t need) {
+  if (need <= *cap && *p) return FGB_OK;
+  if (*p) { cudaFreeHost(*p); *p = nullptr; *cap = 0; }
+  const uint64_t n = need + need / 8 + 64;
+  cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(p), n * sizeof(T), cudaHostAllocDefault);
+  if (e != cudaSuccess) { cuda_fail(h, e, "cudaHostAlloc"); return FGB_ERR_NOMEM; }
+  *cap = n;
+  return FGB_OK;
+}
+
+// Smallest call (unique keys) that takes the enumeration form instead of all-pairs, by k.  Set from the device time
+// of the two forms' edge kernels (CUDA events, scripts/bench_umi_assign.py --crossover; DESIGN.md section 9).
+// FGB_UMI_ENUM_MIN_KEYS overrides both for that measurement.
+uint64_t umi_enum_min_keys(uint32_t k) {
+  if (const char* e = std::getenv("FGB_UMI_ENUM_MIN_KEYS")) return std::strtoull(e, nullptr, 10);
+  return k <= 1 ? 1000 : 8000;
+}
+
+#define FGB_TRY(x) do { fgb_status s__ = (x); if (s__ != FGB_OK) return s__; } while (0)
+
+// Host phase 1 of fgb_umi_assign / fgb_umi_edges: key tables of every call (umi_off is indexed by call_off).
+fgb_status umi_prepare_calls(fgb_handle* h, const fgb_umi_options& o, const uint8_t* umis, const uint64_t* umi_off,
+                             const uint64_t* call_off, uint64_t n_calls, std::vector<fgb_umi::Call>* calls) {
+  calls->assign(n_calls, fgb_umi::Call{});
+  std::vector<std::string> err(n_calls);
+  fgb_umi::parallel_for(n_calls, o.n_threads, [&](uint64_t c) {
+    try {
+      err[c] = fgb_umi::prepare(o, umis, umi_off + call_off[c], call_off[c + 1] - call_off[c], &(*calls)[c]);
+    } catch (const std::bad_alloc&) {
+      err[c] = "out of host memory";
+    }
+  });
+  for (uint64_t c = 0; c < n_calls; ++c)
+    if (!err[c].empty()) {
+      h->last_error = "fgb_umi_assign: call " + std::to_string(c) + ": " + err[c];
+      return err[c] == "out of host memory" ? FGB_ERR_NOMEM : FGB_ERR_INVALID_ARG;
+    }
+  return FGB_OK;
+}
+
+// The device phase: capture lists of every call that can have an edge.  row_base[c] = the call's first CSR row
+// (UINT64_MAX: no device work); the CSR is left in h->umi.h_off (rows + 1 entries) / h->umi.h_edges.
+fgb_status umi_device_edges(fgb_handle* h, const fgb_umi_options& o, const std::vector<fgb_umi::Call>& calls,
+                            std::vector<uint64_t>* row_base_out, float* device_ms) {
+  const uint64_t n_calls = calls.size();
+  const bool bytes = fgb_umi::uses_bytes(o);
+  fgb::UmiCmp cmp{};
+  cmp.k = o.edits;
+  cmp.directed = o.strategy != FGB_UMI_EDIT;
+  cmp.bytes = bytes;
+  cmp.reverse = bytes && o.strategy == FGB_UMI_PAIRED;
+  cmp.zero_ok = o.edits != 1;
+  std::vector<uint64_t>& row_base = *row_base_out;
+  row_base.assign(n_calls, UINT64_MAX);
+  std::vector<uint64_t> enum_calls;
+  std::vector<uint8_t> is_enum(n_calls, 0);
+  uint64_t n_rows = 0, n_blob = 0, n_work = 0, n_sorted = 0, max_sorted = 0;
+  for (uint64_t c = 0; c < n_calls; ++c) {
+    if (!fgb_umi::needs_edges(o, calls[c])) continue;
+    const uint64_t nk = calls[c].keys.size();
+    if (nk > UINT32_MAX) { h->last_error = "fgb_umi_assign: call " + std::to_string(c) + ": too many unique UMIs"; return FGB_ERR_INVALID_ARG; }
+    row_base[c] = n_rows;
+    n_rows += nk;
+    if (bytes) n_blob += calls[c].bytes.size();
+    if (!bytes && o.edits <= 2 && nk >= umi_enum_min_keys(o.edits)) {
+      enum_calls.push_back(c);
+      is_enum[c] = 1;
+      n_sorted += nk;
+      max_sorted = std::max(max_sorted, nk);
+    } else {
+      n_work += (nk + fgb::kUmiThreads - 1) / fgb::kUmiThreads;
+    }
+  }
+  if (device_ms) *device_ms = 0.f;
+  if (!n_rows) return FGB_OK;
+  auto& B = h->umi;
+  std::vector<uint64_t> sorted_base(n_calls, 0);
+  FGB_CUDA(h, cudaSetDevice(h->device));
+  cudaStream_t st = h->slots[0].stream;
+  FGB_TRY(ensure_pinned(h, &B.h_keys, &B.hcap_keys, n_rows));
+  FGB_TRY(ensure_pinned(h, &B.h_blob, &B.hcap_blob, n_blob + 1));
+  FGB_TRY(ensure_pinned(h, &B.h_work, &B.hcap_work, n_work + 1));
+  FGB_TRY(ensure_pinned(h, &B.h_sbits, &B.hcap_sbits, n_sorted + 1));
+  FGB_TRY(ensure_pinned(h, &B.h_sidx, &B.hcap_sidx, n_sorted + 1));
+  FGB_TRY(ensure(h, &B.keys, &B.cap_keys, n_rows));
+  FGB_TRY(ensure(h, &B.blob, &B.cap_blob, n_blob + 1));
+  FGB_TRY(ensure(h, &B.work, &B.cap_work, n_work + 1));
+  FGB_TRY(ensure(h, &B.deg, &B.cap_deg, n_rows + 1));
+  FGB_TRY(ensure(h, &B.off, &B.cap_off, n_rows + 1));
+  FGB_TRY(ensure(h, &B.sbits_in, &B.cap_sbits_in, n_sorted + 1));
+  FGB_TRY(ensure(h, &B.sbits, &B.cap_sbits, n_sorted + 1));
+  FGB_TRY(ensure(h, &B.sidx_in, &B.cap_sidx_in, n_sorted + 1));
+  FGB_TRY(ensure(h, &B.sidx, &B.cap_sidx, n_sorted + 1));
+  if (!B.ev0) {
+    FGB_CUDA(h, cudaEventCreate(&B.ev0));
+    FGB_CUDA(h, cudaEventCreate(&B.ev1));
+    FGB_CUDA(h, cudaEventCreate(&B.ev2));
+    FGB_CUDA(h, cudaEventCreate(&B.ev3));
+  }
+  // stage the tables (string offsets rebased onto the batch's blob) and the all-pairs work list
+  uint64_t w = 0, blob_at = 0, s_at = 0;
+  for (uint64_t c = 0; c < n_calls; ++c) {
+    if (row_base[c] == UINT64_MAX) continue;
+    const auto& cl = calls[c];
+    const uint64_t nk = cl.keys.size();
+    fgb_umi_key* dst = B.h_keys + row_base[c];
+    std::memcpy(dst, cl.keys.data(), nk * sizeof(fgb_umi_key));
+    if (bytes) {
+      for (uint64_t k = 0; k < nk; ++k) dst[k].str_off += blob_at;
+      std::memcpy(B.h_blob + blob_at, cl.bytes.data(), cl.bytes.size());
+      blob_at += cl.bytes.size();
+    }
+    if (is_enum[c]) {
+      sorted_base[c] = s_at;
+      for (uint64_t k = 0; k < nk; ++k) { B.h_sbits[s_at + k] = cl.keys[k].bits; B.h_sidx[s_at + k] = static_cast<uint32_t>(k); }
+      s_at += nk;
+    } else {
+      for (uint64_t q = 0; q < nk; q += fgb::kUmiThreads)
+        B.h_work[w++] = fgb::UmiWork{row_base[c], static_cast<uint32_t>(nk), static_cast<uint32_t>(q)};
+    }
+  }
+  FGB_CUDA(h, cudaMemcpyAsync(B.keys, B.h_keys, n_rows * sizeof(fgb_umi_key), cudaMemcpyHostToDevice, st));
+  if (n_blob) FGB_CUDA(h, cudaMemcpyAsync(B.blob, B.h_blob, n_blob, cudaMemcpyHostToDevice, st));
+  if (n_work) FGB_CUDA(h, cudaMemcpyAsync(B.work, B.h_work, n_work * sizeof(fgb::UmiWork), cudaMemcpyHostToDevice, st));
+  if (n_sorted) {
+    FGB_CUDA(h, cudaMemcpyAsync(B.sbits_in, B.h_sbits, n_sorted * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+    FGB_CUDA(h, cudaMemcpyAsync(B.sidx_in, B.h_sidx, n_sorted * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  }
+  size_t temp_sort = 0, temp_scan = 0;
+  if (max_sorted)
+    FGB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, temp_sort, B.sbits_in, B.sbits, B.sidx_in, B.sidx,
+                                                static_cast<int>(max_sorted), 0, 64, st));
+  FGB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, temp_scan, B.deg, B.off, static_cast<int>(n_rows + 1), st));
+  FGB_TRY(ensure(h, &B.temp, &B.cap_temp, std::max(temp_sort, temp_scan) + 16));
+  // count pass (events bracket the device work: sort, count, scan | fill)
+  FGB_CUDA(h, cudaEventRecord(B.ev0, st));
+  FGB_CUDA(h, cudaMemsetAsync(B.deg + n_rows, 0, sizeof(uint64_t), st));
+  if (n_work) {
+    fgb::umi_pairs_kernel<false><<<static_cast<unsigned>(n_work), fgb::kUmiThreads, 0, st>>>(
+        B.work, B.keys, B.blob, cmp, B.deg, B.off, B.edges);
+    h->launches++;
+  }
+  for (uint64_t c : enum_calls) {
+    const uint64_t nk = calls[c].keys.size(), sb = sorted_base[c];
+    size_t tb = B.cap_temp;
+    FGB_CUDA(h, cub::DeviceRadixSort::SortPairs(B.temp, tb, B.sbits_in + sb, B.sbits + sb, B.sidx_in + sb, B.sidx + sb,
+                                                static_cast<int>(nk), 0, 64, st));
+    fgb::umi_enum_kernel<false><<<static_cast<unsigned>((nk + fgb::kUmiThreads - 1) / fgb::kUmiThreads), fgb::kUmiThreads, 0, st>>>(
+        B.keys + row_base[c], static_cast<uint32_t>(nk), B.sbits + sb, B.sidx + sb, cmp, B.deg + row_base[c], nullptr, nullptr);
+    h->launches += 2;
+  }
+  FGB_CUDA(h, cudaGetLastError());
+  {
+    size_t tb = B.cap_temp;
+    FGB_CUDA(h, cub::DeviceScan::ExclusiveSum(B.temp, tb, B.deg, B.off, static_cast<int>(n_rows + 1), st));
+  }
+  FGB_CUDA(h, cudaEventRecord(B.ev1, st));
+  FGB_TRY(ensure_pinned(h, &B.h_off, &B.hcap_off, n_rows + 1));
+  FGB_CUDA(h, cudaMemcpyAsync(B.h_off, B.off, (n_rows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  FGB_CUDA(h, cudaStreamSynchronize(st));
+  const uint64_t n_edges = B.h_off[n_rows];
+  FGB_TRY(ensure(h, &B.edges, &B.cap_edges, n_edges + 1));
+  FGB_TRY(ensure_pinned(h, &B.h_edges, &B.hcap_edges, n_edges + 1));
+  // fill pass
+  FGB_CUDA(h, cudaEventRecord(B.ev2, st));
+  if (n_work) {
+    fgb::umi_pairs_kernel<true><<<static_cast<unsigned>(n_work), fgb::kUmiThreads, 0, st>>>(
+        B.work, B.keys, B.blob, cmp, B.deg, B.off, B.edges);
+    h->launches++;
+  }
+  for (uint64_t c : enum_calls) {
+    const uint64_t nk = calls[c].keys.size(), sb = sorted_base[c];
+    fgb::umi_enum_kernel<true><<<static_cast<unsigned>((nk + fgb::kUmiThreads - 1) / fgb::kUmiThreads), fgb::kUmiThreads, 0, st>>>(
+        B.keys + row_base[c], static_cast<uint32_t>(nk), B.sbits + sb, B.sidx + sb, cmp, nullptr, B.off + row_base[c], B.edges);
+    h->launches++;
+  }
+  FGB_CUDA(h, cudaGetLastError());
+  FGB_CUDA(h, cudaEventRecord(B.ev3, st));
+  if (n_edges) FGB_CUDA(h, cudaMemcpyAsync(B.h_edges, B.edges, n_edges * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  FGB_CUDA(h, cudaStreamSynchronize(st));
+  if (device_ms) {
+    float a = 0.f, b = 0.f;
+    FGB_CUDA(h, cudaEventElapsedTime(&a, B.ev0, B.ev1));
+    FGB_CUDA(h, cudaEventElapsedTime(&b, B.ev2, B.ev3));
+    *device_ms = a + b;
+  }
+  return FGB_OK;
+}
+
+fgb_status umi_check_layout(fgb_handle* h, const uint64_t* umi_off, uint64_t n_umis, const uint64_t* call_off,
+                            uint64_t n_calls, const uint64_t* group_off, uint64_t n_groups) {
+  auto layout = [&](const char* what) { h->last_error = std::string("fgb_umi_assign: ") + what; return FGB_ERR_INVALID_ARG; };
+  if (group_off[0] != 0 || group_off[n_groups] != n_calls) return layout("group_off must run from 0 to n_calls");
+  if (call_off[0] != 0 || call_off[n_calls] != n_umis) return layout("call_off must run from 0 to n_umis");
+  for (uint64_t g = 0; g < n_groups; ++g) if (group_off[g + 1] < group_off[g]) return layout("group_off descends");
+  for (uint64_t c = 0; c < n_calls; ++c) if (call_off[c + 1] < call_off[c]) return layout("call_off descends");
+  for (uint64_t u = 0; u < n_umis; ++u) if (umi_off[u + 1] < umi_off[u]) return layout("umi_off descends");
+  return FGB_OK;
+}
+
+fgb_status umi_assign_impl(fgb_handle* h, const fgb_umi_options& o, const uint8_t* umis, const uint64_t* umi_off,
+                           uint64_t n_umis, const uint64_t* call_off, uint64_t n_calls, const uint64_t* group_off,
+                           uint64_t n_groups, uint64_t* ids, uint8_t* kinds, uint64_t* group_mi_count) {
+  FGB_TRY(umi_check_layout(h, umi_off, n_umis, call_off, n_calls, group_off, n_groups));
+  // 1. unique / count / sort per call on the host threads
+  std::vector<fgb_umi::Call> calls;
+  const auto t0 = std::chrono::steady_clock::now();
+  FGB_TRY(umi_prepare_calls(h, o, umis, umi_off, call_off, n_calls, &calls));
+  const auto t1 = std::chrono::steady_clock::now();
+  // 2. the device: capture lists of every call that can have an edge
+  std::vector<uint64_t> row_base;
+  float dev_ms = 0.f;
+  FGB_TRY(umi_device_edges(h, o, calls, &row_base, &dev_ms));
+  const auto t2 = std::chrono::steady_clock::now();
+  auto& B = h->umi;
+  // 3. the order-dependent rules per call, in parallel across calls
+  fgb_umi::parallel_for(n_calls, o.n_threads, [&](uint64_t c) {
+    const bool dev = row_base[c] != UINT64_MAX;
+    fgb_umi::resolve(o, calls[c], dev ? B.h_off + row_base[c] : nullptr, dev ? B.h_edges : nullptr,
+                     ids + call_off[c], kinds + call_off[c]);
+  });
+  // 4. numbering across a group's calls: mapped assigners keep one counter, unmapped ones restart at 0
+  for (uint64_t g = 0; g < n_groups; ++g) {
+    uint64_t base = 0, count = 0;
+    for (uint64_t c = group_off[g]; c < group_off[g + 1]; ++c) {
+      uint64_t taken = 0;
+      for (uint64_t u = call_off[c]; u < call_off[c + 1]; ++u) {
+        if (kinds[u] == FGB_MOL_NONE) continue;
+        taken = std::max(taken, ids[u] + 1);
+        if (o.rules == FGB_UMI_RULES_MAPPED) ids[u] += base;
+        count = std::max(count, ids[u] + 1);
+      }
+      if (o.rules == FGB_UMI_RULES_MAPPED) base += taken;
+    }
+    group_mi_count[g] = count;
+  }
+  const auto t3 = std::chrono::steady_clock::now();
+  auto ms = [](auto a, auto b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
+  B.timing[0] = ms(t0, t1);
+  B.timing[1] = ms(t1, t2);
+  B.timing[2] = dev_ms;
+  B.timing[3] = ms(t2, t3);
+  return FGB_OK;
+}
+
+// No exception crosses the ABI: host allocations (and thread creation) that fail become status codes.
+template <class F>
+fgb_status umi_guard(fgb_handle* h, F&& f) {
+  try {
+    return f();
+  } catch (const std::bad_alloc&) {
+    h->last_error = "fgb_umi_assign: out of host memory";
+    return FGB_ERR_NOMEM;
+  } catch (const std::exception& e) {
+    h->last_error = std::string("fgb_umi_assign: ") + e.what();
+    return FGB_ERR_NOMEM;
+  }
+}
+
+}  // namespace
+
+extern "C" {
+
+fgb_status fgb_umi_assign(fgb_handle* h, const fgb_umi_options* opt, const uint8_t* umis, const uint64_t* umi_off,
+                          uint64_t n_umis, const uint64_t* call_off, uint64_t n_calls, const uint64_t* group_off,
+                          uint64_t n_groups, uint64_t* ids, uint8_t* kinds, uint64_t* group_mi_count) {
+  if (!h || !opt || !umi_off || !call_off || !group_off || (n_umis && (!umis || !ids || !kinds)) ||
+      (n_groups && !group_mi_count))
+    return FGB_ERR_INVALID_ARG;
+  const std::string bad = fgb_umi::check_options(*opt);
+  if (!bad.empty()) { h->last_error = "fgb_umi_assign: " + bad; return FGB_ERR_INVALID_ARG; }
+  if (h->submit_pending) { h->last_error = "fgb_umi_assign: a submit has not been waited on"; return FGB_ERR_BUSY; }
+  return umi_guard(h, [&] {
+    return umi_assign_impl(h, *opt, umis, umi_off, n_umis, call_off, n_calls, group_off, n_groups, ids, kinds,
+                           group_mi_count);
+  });
+}
+
+fgb_status fgb_umi_last_timing(const fgb_handle* h, double ms[4]) {
+  if (!h || !ms) return FGB_ERR_INVALID_ARG;
+  std::memcpy(ms, h->umi.timing, sizeof(h->umi.timing));
+  return FGB_OK;
+}
+
+fgb_status fgb_umi_edges(fgb_handle* h, const fgb_umi_options* opt, const uint8_t* umis, const uint64_t* umi_off,
+                         uint64_t n_umis, uint64_t* n_keys, uint64_t* edge_off, uint32_t* edges, uint64_t cap,
+                         uint64_t* n_edges) {
+  if (!h || !opt || !umi_off || !n_keys || !edge_off || !n_edges || (n_umis && !umis)) return FGB_ERR_INVALID_ARG;
+  const std::string bad = fgb_umi::check_options(*opt);
+  if (!bad.empty()) { h->last_error = "fgb_umi_edges: " + bad; return FGB_ERR_INVALID_ARG; }
+  if (h->submit_pending) { h->last_error = "fgb_umi_edges: a submit has not been waited on"; return FGB_ERR_BUSY; }
+  return umi_guard(h, [&]() -> fgb_status {
+    const uint64_t call_off[2] = {0, n_umis}, group_off[2] = {0, 1};
+    FGB_TRY(umi_check_layout(h, umi_off, n_umis, call_off, 1, group_off, 1));
+    std::vector<fgb_umi::Call> calls;
+    FGB_TRY(umi_prepare_calls(h, *opt, umis, umi_off, call_off, 1, &calls));
+    std::vector<uint64_t> row_base;
+    FGB_TRY(umi_device_edges(h, *opt, calls, &row_base, nullptr));
+    const uint64_t nk = calls[0].keys.size();
+    *n_keys = nk;
+    if (row_base[0] == UINT64_MAX) {   // nothing for the device: no edges
+      std::fill(edge_off, edge_off + nk + 1, 0);
+      *n_edges = 0;
+      return FGB_OK;
+    }
+    const uint64_t* o = h->umi.h_off + row_base[0];
+    for (uint64_t k = 0; k <= nk; ++k) edge_off[k] = o[k] - o[0];
+    *n_edges = o[nk] - o[0];
+    if (edges && cap >= *n_edges && *n_edges) std::memcpy(edges, h->umi.h_edges + o[0], *n_edges * sizeof(uint32_t));
+    return FGB_OK;
+  });
+}
 
 }  // extern "C"

@@ -187,6 +187,22 @@ class FgbCallerOptions(C.Structure):
     ]
 
 
+FGB_UMI_IDENTITY, FGB_UMI_EDIT, FGB_UMI_ADJACENCY, FGB_UMI_PAIRED = 0, 1, 2, 3
+FGB_UMI_RULES_MAPPED, FGB_UMI_RULES_UNMAPPED = 0, 1
+FGB_MOL_NONE, FGB_MOL_SINGLE, FGB_MOL_A, FGB_MOL_B = 0, 1, 2, 3
+
+
+class FgbUmiOptions(C.Structure):
+    _fields_ = [("strategy", C.c_uint32), ("edits", C.c_uint32), ("rules", C.c_uint32),
+                ("min_umi_length", C.c_uint32), ("n_threads", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class FgbUmiKey(C.Structure):
+    _fields_ = [("bits", C.c_uint64), ("str_off", C.c_uint64), ("str_len", C.c_uint32), ("count", C.c_uint32),
+                ("first", C.c_uint32), ("dash", C.c_uint32), ("len", C.c_uint8), ("flags", C.c_uint8),
+                ("reserved", C.c_uint8 * 6)]
+
+
 FGB_NSTATS = 24
 STAT_NAMES = ("total_reads", "consensus_reads", "filtered_reads", "InsufficientReads",
               "SecondaryOrSupplementary", "ZeroLengthAfterTrimming", "MinorityAlignment",
@@ -212,6 +228,8 @@ SYMBOLS = (
     "fgb_caller_flush", "fgb_caller_take_rejects", "fgb_caller_stats", "fgb_overlap_apply_group", "fgb_pack8_encode",
     "fgb_submit_pack8", "fgb_submit_bam4", "fgb_unpack_bam4_device", "fgb_unpack_records_device", "fgb_submit_ex", "fgb_filter_simplex_device", "fgb_struct_size", "fgb_caller_add_groups", "fgb_filter_record", "fgb_host_is_fr_pair",
     "fgb_host_num_bases_extending_past_mate", "fgb_host_clip_cigar_ops", "fgb_host_read_pos_at_ref_pos", "fgb_host_simplify_cigar", "fgb_host_source_reads", "fgb_host_consensus_umis", "fgb_caller_pending", "fgb_host_simplex_record", "fgb_bgzf_bound", "fgb_bgzf_compress", "fgb_bgzf_scan_members", "fgb_bgzf_inflate_device", "fgb_host_inflate_member", "fgb_bam_header", "fgb_bgzf_uncompressed_size", "fgb_bgzf_decompress", "fgb_bam_read_header", "fgb_bam_split_records", "fgb_host_group_by_mi", "fgb_host_duplex_record",
+    "fgb_umi_assign", "fgb_host_umi_for_read", "fgb_host_umi_prepare", "fgb_host_umi_resolve",
+    "fgb_umi_edges", "fgb_umi_last_timing",
 )
 
 _lib = None
@@ -379,6 +397,20 @@ def load() -> C.CDLL:
     lib.fgb_caller_pending.restype = C.c_int32
     lib.fgb_caller_add_groups.argtypes = [vp, vp, vp, vp, u64]
     lib.fgb_caller_add_groups.restype = C.c_int32
+    lib.fgb_umi_assign.argtypes = [vp, C.POINTER(FgbUmiOptions), vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
+    lib.fgb_umi_assign.restype = C.c_int32
+    lib.fgb_host_umi_for_read.argtypes = [C.POINTER(FgbUmiOptions), C.c_char_p, C.c_size_t, C.c_int, vp, C.c_size_t,
+                                          C.POINTER(C.c_size_t)]
+    lib.fgb_host_umi_for_read.restype = C.c_int32
+    lib.fgb_host_umi_prepare.argtypes = [C.POINTER(FgbUmiOptions), vp, vp, u64, vp, C.POINTER(u64), vp, vp]
+    lib.fgb_host_umi_prepare.restype = C.c_int32
+    lib.fgb_host_umi_resolve.argtypes = [C.POINTER(FgbUmiOptions), vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, vp]
+    lib.fgb_host_umi_resolve.restype = C.c_int32
+    lib.fgb_umi_edges.argtypes = [vp, C.POINTER(FgbUmiOptions), vp, vp, u64, C.POINTER(u64), vp, vp, u64,
+                                  C.POINTER(u64)]
+    lib.fgb_umi_edges.restype = C.c_int32
+    lib.fgb_umi_last_timing.argtypes = [vp, vp]
+    lib.fgb_umi_last_timing.restype = C.c_int32
     lib.fgb_struct_size.argtypes = [C.c_uint32]
     lib.fgb_struct_size.restype = C.c_uint32
     _lib = lib

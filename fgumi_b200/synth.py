@@ -250,3 +250,25 @@ def record_families(n_families: int, depth: int = 8, L: int = 150, error_rate: f
     rec_off = np.arange(R + 1, dtype=np.uint64) * np.uint64(rec_len)
     group_rec = np.arange(U + 1, dtype=np.uint64) * np.uint64(D)
     return rec.reshape(-1), rec_off, group_rec
+
+
+def umi_families(n_molecules: int, length: int, mean_family: float = 4.0, error_rate: float = 0.01,
+                 paired: bool = False, swap_rate: float = 0.5, seed: int = 0):
+    """Seeded UMIs of one position group: `n_molecules` true UMIs of `length` bases, family sizes 1 + Poisson
+    (mean_family - 1), each base of each read's UMI replaced by another base with probability `error_rate`.
+    With `paired` a true UMI is "X-Y" (two halves of `length` bases) and a read of the other strand carries
+    "Y-X" with probability `swap_rate`.  Returns a list of str, reads in random order."""
+    rng = np.random.default_rng(seed)
+    L = length * 2 if paired else length
+    true = rng.integers(0, 4, size=(n_molecules, L), dtype=np.uint8)
+    sizes = 1 + rng.poisson(max(mean_family - 1.0, 0.0), size=n_molecules)
+    reads = np.repeat(true, sizes, axis=0)
+    err = rng.random(reads.shape) < error_rate
+    reads = np.where(err, (reads + rng.integers(1, 4, size=reads.shape, dtype=np.uint8)) % 4, reads)
+    reads = reads[rng.permutation(len(reads))]
+    txt = ACGT[reads]
+    out = [bytes(r).decode() for r in txt]
+    if paired:
+        swap = rng.random(len(out)) < swap_rate
+        out = [(u[length:] + "-" + u[:length]) if s else (u[:length] + "-" + u[length:]) for u, s in zip(out, swap)]
+    return out

@@ -818,6 +818,78 @@ fgb_status fgb_caller_flush(fgb_caller* c, const uint8_t** out_data, uint64_t* o
                             uint64_t* out_count);
 fgb_status fgb_caller_stats(const fgb_caller* c, uint64_t stats[FGB_NSTATS]);
 
+/* ---- UMI assignment: the four `fgumi group` strategies (crates/fgumi-umi/src/assigner.rs for mapped data,
+ * src/lib/umi/parallel_assigner.rs for `group --allow-unmapped`) ---------------------------------------------
+ * A batch of position groups; group g is calls [group_off[g], group_off[g+1]), call c is UMIs
+ * [call_off[c], call_off[c+1]), UMI u is bytes [umi_off[u], umi_off[u+1]) of `umis` (what umi_for_read made of
+ * the read's tag: fgb_host_umi_for_read).  A call is one UmiAssigner::assign (the orientation sub-groups of a
+ * position group are separate calls, group.rs:382-407).  Per UMI the result is a kind (FGB_MOL_*) and an id
+ * LOCAL to its group: mapped rules keep one counter across a group's calls, unmapped rules restart at 0 on
+ * every call.  group_mi_count[g] = max(id) + 1 over the group (0 if nothing is assigned), so the MI of a UMI is
+ * "N", "N/A" or "N/B" with N = id + the sum of the earlier groups' counts + the run's base.
+ * The device finds the UMI graph's edges (umi_kernels.cuh); unique / count / sort and the order-dependent rules
+ * (BFS from roots in sorted order, union-find, numbering) run on n_threads host threads. */
+enum { FGB_UMI_IDENTITY = 0, FGB_UMI_EDIT = 1, FGB_UMI_ADJACENCY = 2, FGB_UMI_PAIRED = 3 };
+enum { FGB_UMI_RULES_MAPPED = 0, FGB_UMI_RULES_UNMAPPED = 1 };
+enum { FGB_MOL_NONE = 0, FGB_MOL_SINGLE = 1, FGB_MOL_A = 2, FGB_MOL_B = 3 };
+typedef struct fgb_umi_options {
+  uint32_t strategy;        /* FGB_UMI_*                                                                 */
+  uint32_t edits;           /* max mismatches; must be 0 for identity                                    */
+  uint32_t rules;           /* FGB_UMI_RULES_*                                                           */
+  uint32_t min_umi_length;  /* 0 = none; else every UMI of a call is truncated to it, a shorter one fails */
+  uint32_t n_threads;       /* host threads; 0 or 1 = the calling thread only                           */
+  uint32_t reserved;
+} fgb_umi_options;
+/* Errors fail the whole batch with FGB_ERR_INVALID_ARG and fgb_last_error names the call: valid UMIs of different
+ * base lengths in one mapped adjacency call, a paired UMI without exactly one '-', a UMI shorter than
+ * min_umi_length, edits != 0 with identity, malformed offsets.  ids / kinds hold n_umis entries. */
+fgb_status fgb_umi_assign(fgb_handle* h, const fgb_umi_options* opt, const uint8_t* umis, const uint64_t* umi_off,
+                          uint64_t n_umis, const uint64_t* call_off, uint64_t n_calls, const uint64_t* group_off,
+                          uint64_t n_groups, uint64_t* ids, uint8_t* kinds, uint64_t* group_mi_count);
+/* umi_for_read (group.rs:300-350): the upper-cased UMI, or for mapped paired rules the prefixed form
+ * "a..a:<first>-b..b:<second>" (prefixes of edits + 1 characters; swapped when R2 is earlier).  Host code. */
+fgb_status fgb_host_umi_for_read(const fgb_umi_options* opt, const uint8_t* umi, size_t len, int is_r1_earlier,
+                                 uint8_t* out, size_t cap, size_t* out_len);
+/* The unique-key table of one call as fgb_umi_assign sends it to the device, in the order the rules sort it:
+ * identity and mapped edit by string, unmapped edit by first appearance, adjacency and paired by count
+ * descending then string.  Exposed with fgb_host_umi_resolve so the host half can be tested without a device. */
+typedef struct fgb_umi_key {
+  uint64_t bits;            /* BitEnc (bitenc.rs:32-90): base i in bits 2i..2i+1, A=0 C=1 G=2 T=3         */
+  uint64_t str_off;         /* the key's string in key_bytes                                             */
+  uint32_t str_len;
+  uint32_t count;           /* UMIs of the call with this key                                            */
+  uint32_t first;           /* index within the call of its first UMI                                    */
+  uint32_t dash;            /* position of the '-' (paired keys)                                         */
+  uint8_t len;              /* bases in bits                                                             */
+  uint8_t flags;            /* FGB_UMI_KEY_LAST: the last key of its BitEnc (unmapped rules look BitEncs
+                               up in a map where the last index wins, parallel_assigner.rs:184-185)      */
+  uint8_t reserved[6];
+} fgb_umi_key;
+enum { FGB_UMI_KEY_LAST = 1 };
+/* keys has room for n_umis entries, key_bytes for umi_off[n_umis] - umi_off[0] bytes, key_of for n_umis
+ * (UINT32_MAX: the UMI has no key). */
+fgb_status fgb_host_umi_prepare(const fgb_umi_options* opt, const uint8_t* umis, const uint64_t* umi_off,
+                                uint64_t n_umis, fgb_umi_key* keys, uint64_t* n_keys, uint8_t* key_bytes,
+                                uint32_t* key_of);
+/* The rules of one call given its key table and capture lists (key i's neighbours edges[edge_off[i] ..
+ * edge_off[i+1]), ascending): ids from 0 as a fresh assigner would give them. */
+fgb_status fgb_host_umi_resolve(const fgb_umi_options* opt, const uint8_t* umis, const uint64_t* umi_off,
+                                uint64_t n_umis, const fgb_umi_key* keys, uint64_t n_keys, const uint8_t* key_bytes,
+                                const uint32_t* key_of, const uint64_t* edge_off, const uint32_t* edges,
+                                uint64_t* ids, uint8_t* kinds);
+
+/* The capture lists the device finds for ONE call, as fgb_umi_assign computes them (the CSR fgb_host_umi_resolve
+ * takes): *n_keys keys (the order of fgb_host_umi_prepare), edge_off[0 .. *n_keys] (room for n_umis + 1 entries),
+ * *n_edges entries, written to `edges` only when cap >= *n_edges (call with cap 0 to size).  For tests and for
+ * integrations that apply their own rules to the graph. */
+fgb_status fgb_umi_edges(fgb_handle* h, const fgb_umi_options* opt, const uint8_t* umis, const uint64_t* umi_off,
+                         uint64_t n_umis, uint64_t* n_keys, uint64_t* edge_off, uint32_t* edges, uint64_t cap,
+                         uint64_t* n_edges);
+/* Where the last fgb_umi_assign on this handle spent its time, in ms: [0] key tables on the host, [1] the device
+ * phase as the host saw it (staging, copies, kernels), [2] the edge kernels alone (CUDA events around the count
+ * pass with its sort / scan and around the fill pass), [3] the rules and numbering on the host. */
+fgb_status fgb_umi_last_timing(const fgb_handle* h, double ms[4]);
+
 /* sizeof() of the ABI structs as this library was compiled, so a binding can check its own layout:
  * 0 fgb_caller_options, 1 fgb_filter_params, 2 fgb_submit_options, 3 fgb_raw_columns,
  * 4 fgb_raw_read, 5 fgb_batch, 6 fgb_codec_params, 7 fgb_params, 8 fgb_duplex_filter_params,
