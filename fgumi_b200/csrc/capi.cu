@@ -203,6 +203,24 @@ fgb_status launch_vote(fgb_handle* h, const fgb_batch& b, const fgb_columns& out
   return FGB_OK;
 }
 
+// The device pointers the vote kernels can use: bulk copies (cp.async.bulk) read bases, quals, reads and units from
+// 16-byte aligned addresses, tiles are read as 16-byte words, and the outputs are written 8 positions at a time
+// (8-byte words of base / qual, 16-byte words of depth / errors).  Checked before anything is enqueued.
+fgb_status check_vote_pointers(fgb_handle* h, const fgb_batch& b, const fgb_columns& out, const char* who) {
+  if (b.n_tiles == 0) return FGB_OK;
+  const struct { const void* p; uintptr_t align; const char* name; } ptrs[] = {
+      {b.bases, 16, "bases"}, {b.quals, 16, "quals"}, {b.reads, 16, "reads"}, {b.units, 16, "units"},
+      {b.tiles, 16, "tiles"}, {out.base, 8, "output base"}, {out.qual, 8, "output qual"},
+      {out.depth, 16, "output depth"}, {out.errors, 16, "output errors"}};
+  for (const auto& x : ptrs) {
+    if (reinterpret_cast<uintptr_t>(x.p) % x.align) {
+      h->last_error = std::string(who) + ": " + x.name + " is not " + std::to_string(x.align) + "-byte aligned";
+      return FGB_ERR_LAYOUT;
+    }
+  }
+  return FGB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -525,6 +543,8 @@ fgb_status fgb_vote_device(fgb_handle* h, const fgb_batch* in, const fgb_columns
   if (in->n_tiles && (!in->tiles || !in->units || !out->base || !out->qual || !out->depth ||
                       !out->errors))
     return FGB_ERR_INVALID_ARG;
+  fgb_status st = check_vote_pointers(h, *in, *out, "fgb_vote_device");
+  if (st != FGB_OK) return st;
   FGB_CUDA(h, cudaSetDevice(h->device));
   return launch_vote(h, *in, *out, static_cast<cudaStream_t>(stream));
 }
@@ -1226,14 +1246,15 @@ fgb_status fgb_vote_duplex_device(fgb_handle* h, const fgb_batch* in, const fgb_
   if (!h || !in || !ss || !out || (n_jobs && !jobs)) return FGB_ERR_INVALID_ARG;
   if (in->n_tiles && (!in->tiles || !in->units || !ss->base || !ss->qual || !ss->depth || !ss->errors))
     return FGB_ERR_INVALID_ARG;
+  fgb_status vst = check_vote_pointers(h, *in, *ss, "fgb_vote_duplex_device");
+  if (vst != FGB_OK) return vst;
   FGB_CUDA(h, cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   // the epilogue moves 8 elements at a time: byte columns 8-byte aligned, u16 columns and job records 16-byte aligned
-  const uintptr_t align8 = reinterpret_cast<uintptr_t>(ss->base) | reinterpret_cast<uintptr_t>(ss->qual) |
-                           reinterpret_cast<uintptr_t>(out->base) | reinterpret_cast<uintptr_t>(out->qual) |
-                           reinterpret_cast<uintptr_t>(tile_jobs) | reinterpret_cast<uintptr_t>(in->bases);
-  const uintptr_t align16 = reinterpret_cast<uintptr_t>(ss->depth) | reinterpret_cast<uintptr_t>(out->errors) |
-                            reinterpret_cast<uintptr_t>(jobs);
+  // (the batch and the SS columns passed check_vote_pointers; what is left are the pointers only the epilogue uses)
+  const uintptr_t align8 = reinterpret_cast<uintptr_t>(out->base) | reinterpret_cast<uintptr_t>(out->qual) |
+                           reinterpret_cast<uintptr_t>(tile_jobs);
+  const uintptr_t align16 = reinterpret_cast<uintptr_t>(out->errors) | reinterpret_cast<uintptr_t>(jobs);
   const bool fused = n_jobs && in->n_tiles && tile_jobs && job_index && (align8 & 7u) == 0 && (align16 & 15u) == 0;
   if (!fused) {
     fgb_status st = launch_vote(h, *in, *ss, s);

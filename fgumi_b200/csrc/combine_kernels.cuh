@@ -64,7 +64,10 @@ __device__ __forceinline__ DuplexJobRegs load_duplex_job(const DuplexArgs& a, ui
 
 // One job on one warp: every arm of duplex_consensus, any row length, any alignment.  It is the whole of the fallback
 // kernel and the redo path of the word kernel below (single-strand arms, rows that are not 8-aligned, more than 255
-// pooled source reads).
+// pooled source reads).  `WordsOk`: the column pointers are aligned for 8-byte / 16-byte accesses (the word kernels
+// only launch on such columns); the fallback kernel runs on columns that are not and passes false, which leaves the
+// byte / u16 path alone.
+template <bool WordsOk>
 __device__ __forceinline__ uint8_t duplex_job_warp(const DuplexArgs& a, const DuplexJobRegs& cur, uint32_t lane) {
   const fgb_duplex_job job = cur.job;
   const fgb_unit ua = cur.ua, ub = cur.ub;
@@ -72,9 +75,10 @@ __device__ __forceinline__ uint8_t duplex_job_warp(const DuplexArgs& a, const Du
   const uint32_t len = la < lb ? la : lb;                       // duplex_caller.rs:846-849
   const uint32_t ra0 = ua.read_begin, ra1 = cur.ra1;
   const uint32_t rb0 = ub.read_begin, rb1 = cur.rb1;
-  // Word path: 8 positions per lane with byte-parallel arithmetic.  Needs 8-aligned rows (the layout rule
-  // for inputs; job.out_off is the caller's) and per-position error counts that fit a byte.
-  const bool words = ((ua.out_off | ub.out_off | job.out_off) & 7u) == 0 && (ra1 - ra0) + (rb1 - rb0) <= 255u;
+  // Word path: 8 positions per lane with byte-parallel arithmetic.  Needs aligned column pointers, 8-aligned rows
+  // (the layout rule for inputs; job.out_off is the caller's) and per-position error counts that fit a byte.
+  const bool words = WordsOk && ((ua.out_off | ub.out_off | job.out_off) & 7u) == 0 &&
+                     (ra1 - ra0) + (rb1 - rb0) <= 255u;
   uint8_t status;
   if (words && len <= 256u) {
     // ---- one block per job (reads up to 256 bases): everything the job needs is requested at once ----
@@ -295,6 +299,7 @@ __device__ __forceinline__ uint8_t duplex_job_warp(const DuplexArgs& a, const Du
   return status;
 }
 
+// Fallback kernel: one warp per job, byte / u16 accesses (column pointers that are not aligned for the word kernel).
 __global__ void __launch_bounds__(kCombineThreads) duplex_combine_kernel(const DuplexArgs a) {
   const uint32_t lane = threadIdx.x & 31u;
   const uint64_t warp0 = static_cast<uint64_t>(blockIdx.x) * kCombineJobsPerCta + (threadIdx.x >> 5);
@@ -305,7 +310,7 @@ __global__ void __launch_bounds__(kCombineThreads) duplex_combine_kernel(const D
   for (uint64_t j = warp0; j < a.n_jobs; j += wstride) {
     const DuplexJobRegs cur = nx;
     if (j + wstride < a.n_jobs) nx = load_duplex_job(a, j + wstride);
-    const uint8_t status = duplex_job_warp(a, cur, lane);
+    const uint8_t status = duplex_job_warp<false>(a, cur, lane);
     if (lane == 0) {
       if (a.out_status) a.out_status[j] = status;
       ++done;
@@ -474,7 +479,7 @@ __device__ __forceinline__ void duplex_combine_words_chunk(const DuplexArgs& a, 
     const uint32_t f = s_any[jl];
     const bool general = sj[jl].general != 0u;
     uint8_t status = f == 3u ? FGB_DUPLEX_BOTH : FGB_DUPLEX_NONE;
-    if (general || f == 1u || f == 2u) status = duplex_job_warp(a, load_duplex_job(a, j0 + jl), lane);
+    if (general || f == 1u || f == 2u) status = duplex_job_warp<true>(a, load_duplex_job(a, j0 + jl), lane);
     if (lane == 0 && a.out_status) a.out_status[j0 + jl] = status;
   }
 }

@@ -203,7 +203,11 @@ fgb_status fgb_sort_tiles_by_class(fgb_tile* tiles, uint64_t n_tiles, uint64_t c
 /* ---- the vote (simplex / single-strand consensus), K1 --------------------------------- */
 /* Device-resident form: every pointer in `in`/`out` is a DEVICE pointer on the handle's GPU.
  * Enqueues ONE kernel launch on `stream` (a cudaStream_t passed as void*; NULL = default
- * stream) that calls every position of every unit.  Asynchronous. */
+ * stream) that calls every position of every unit.  Asynchronous.
+ * Pointer alignment (the kernels read their inputs with bulk copies and write 8 positions at a time):
+ * in->bases, in->quals, in->reads, in->units and in->tiles 16-byte aligned; out->base and out->qual 8-byte
+ * aligned; out->depth and out->errors 16-byte aligned.  Anything else returns FGB_ERR_LAYOUT (fgb_last_error
+ * names the pointer) and enqueues nothing. */
 fgb_status fgb_vote_device(fgb_handle* h, const fgb_batch* in, const fgb_columns* out,
                            void* stream);
 
@@ -545,13 +549,18 @@ fgb_status fgb_plan_tiles_jobs(const fgb_unit* units, uint64_t n_units, const fg
 /* Vote `in` (tiles from fgb_plan_tiles_jobs, class_tiles set) into `ss` and combine `jobs` into `out`: attached
  * both-strand jobs in the vote's epilogue, every other job (single-strand arms, unattached jobs, rows that are
  * not 8-aligned) by the standalone kernels afterwards.  Results are those of fgb_vote_device followed by
- * fgb_duplex_combine_device, bit for bit.  All pointers are device pointers; tile_jobs has in->n_tiles entries. */
+ * fgb_duplex_combine_device, bit for bit.  All pointers are device pointers; tile_jobs has in->n_tiles entries.
+ * `in` and `ss` follow fgb_vote_device's alignment rule (FGB_ERR_LAYOUT otherwise, nothing enqueued).  The
+ * combine runs in the epilogue only when out->base, out->qual and tile_jobs are 8-byte aligned and out->errors and
+ * jobs 16-byte aligned; otherwise the call is fgb_vote_device followed by fgb_duplex_combine_device. */
 fgb_status fgb_vote_duplex_device(fgb_handle* h, const fgb_batch* in, const fgb_columns* ss,
                                   const fgb_duplex_job* jobs, uint64_t n_jobs,
                                   const fgb_tile_jobs* tile_jobs, const uint32_t* job_index,
                                   const fgb_duplex_out* out, void* stream);
 
-/* `ss` are the four single-strand columns the vote wrote for `in` (device pointers). */
+/* `ss` are the four single-strand columns the vote wrote for `in` (device pointers).  Any column alignment: when
+ * in->bases, ss->base, ss->qual, out->base and out->qual are 8-byte aligned and ss->depth and out->errors 16-byte
+ * aligned a word kernel runs, otherwise a kernel with one warp per job and byte / u16 accesses. */
 fgb_status fgb_duplex_combine_device(fgb_handle* h, const fgb_batch* in, const fgb_columns* ss,
                                      const fgb_duplex_job* jobs, uint64_t n_jobs,
                                      const fgb_duplex_out* out, void* stream);

@@ -62,6 +62,13 @@ dp += [(4 * m, 4 * (m + 30) + 1) for m in range(0, 80, 9)]
 _duplex_against_oracle(fg, du, dp, True)
 du, dp = _duplex_molecules(rng, 200)
 _duplex_against_oracle(fg, du, dp, True)
+# the fallback kernels of K4, K2 and K3 (column pointers that are not aligned for the word kernels)
+from tests.test_fallback_kernels import FILTER_GRID, codec_forms, duplex_forms, filter_forms
+filter_forms(fg, FILTER_GRID[0], 11, set())
+du, dp = _duplex_molecules(rng, 40, iupac=True)
+dp.append((5, 5))
+duplex_forms(fg, du, dp)
+codec_forms(fg, 78)
 # K0z: BGZF members inflated on the device (good and damaged members)
 from tests.test_bgzf import test_bgzf_members_inflated_on_the_device
 test_bgzf_members_inflated_on_the_device()

@@ -350,17 +350,10 @@ def _codec_job_reference(L, cols, ua, ub, job, cp):
     return ob, oq, od, oe, nb.value, nd.value
 
 
-def test_codec_combine_generic_jobs(fg):
-    """Every orientation combination, arbitrary pads (strands may stick out of the consensus), lengths from 0 to
-    beyond a thousand, output rows that are not 8-aligned (scalar jobs inside a word-kernel launch), single-strand
-    columns with bases outside A/C/G/T/N (redo path), large depths / errors (u16 wrap-around): the kernel against the
-    oracle's padded combine + mask with orientation done in numpy."""
-    import torch
-    L = O.load()
-    L.orc_codec_combine.restype = None
-    L.orc_codec_mask.restype = None
-    rng = np.random.default_rng(77)
-    dev = "cuda:0"
+def _codec_job_mix(fg, rng):
+    """A unit table, CODEC jobs and single-strand host columns: every orientation combination, arbitrary pads, lengths
+    from 0 to 1300, some output rows that are not 8-aligned, a few bases outside A/C/G/T/N and large depths / errors.
+    Returns (units, jobs, (base, qual, depth, errors), output elements the jobs' rows span)."""
     n_jobs = 32 * 9 + 5
     UNIT = np.dtype([("out_off", "<u8"), ("read_begin", "<u4"), ("cons_len", "<u4")])
     units = np.zeros(2 * n_jobs + 1, dtype=UNIT)
@@ -404,7 +397,23 @@ def test_codec_combine_generic_jobs(fg):
             o, l = int(units[2 * m]["out_off"]), int(units[2 * m]["cons_len"])
             if l:
                 sb[o + int(rng.integers(0, l))] = rng.choice(np.frombuffer(b"acgtnRY", np.uint8))
-    ss = fg.DeviceColumns(off + 16, dev)
+    return units, jobs, (sb, sq, sd, se), ooff
+
+
+def test_codec_combine_generic_jobs(fg):
+    """Every orientation combination, arbitrary pads (strands may stick out of the consensus), lengths from 0 to
+    beyond a thousand, output rows that are not 8-aligned (scalar jobs inside a word-kernel launch), single-strand
+    columns with bases outside A/C/G/T/N (redo path), large depths / errors (u16 wrap-around): the kernel against the
+    oracle's padded combine + mask with orientation done in numpy."""
+    import torch
+    L = O.load()
+    L.orc_codec_combine.restype = None
+    L.orc_codec_mask.restype = None
+    rng = np.random.default_rng(77)
+    dev = "cuda:0"
+    units, jobs, (sb, sq, sd, se), ooff = _codec_job_mix(fg, rng)
+    n_jobs = len(jobs)
+    ss = fg.DeviceColumns(len(sb), dev)
     ss.base.copy_(torch.from_numpy(sb)); ss.qual.copy_(torch.from_numpy(sq))
     ss.depth.copy_(torch.from_numpy(sd.view(np.int16))); ss.errors.copy_(torch.from_numpy(se.view(np.int16)))
     db = _UnitsOnly(fg, units, dev)
