@@ -130,3 +130,121 @@ def simplex_file(in_path: str, out_path: str, caller, n_threads: int = 4, level:
                "groups": float(len(groups) - 1), "consensus_reads": float(cnt.value), "output_bytes": float(len(payload)),
                "output_compressed_bytes": float(cn.value)})
     return tm
+
+
+def group_header(input_text: bytes, command_line: str = "fgumi_b200 group") -> bytes:
+    """The input header with one @PG appended, chained by PP to the last program of the input's chain
+    (header.rs:136-144): the last @PG no other @PG names as PP; its ID made unique with .1, .2, ..."""
+    lines = input_text.decode("utf-8", "replace").rstrip("\n").split("\n") if input_text else []
+    pgs = [dict(f.split(":", 1) for f in ln.split("\t")[1:] if ":" in f) for ln in lines if ln.startswith("@PG")]
+    ids = [p.get("ID") for p in pgs]
+    referenced = {p.get("PP") for p in pgs}
+    last = next((i for i in reversed(ids) if i not in referenced), ids[-1] if ids else None)
+    uid, k = "fgumi_b200", 0
+    while uid in ids:
+        k += 1
+        uid = "fgumi_b200.%d" % k
+    pg = "@PG\tID:%s\tPN:fgumi_b200" % uid + ("\tPP:%s" % last if last else "") + "\tCL:" + command_line
+    return ("\n".join([ln for ln in lines if ln] + [pg]) + "\n").encode()
+
+
+def check_group_sort_order(text: bytes, allow_unmapped: bool) -> None:
+    """group.rs:797-817: template-coordinate input (SO:unsorted GO:query, SS ending in template-coordinate if
+    present), or queryname-sorted input with --allow-unmapped."""
+    hd = next((ln for ln in text.decode("utf-8", "replace").split("\n") if ln.startswith("@HD")), "")
+    f = dict(x.split(":", 1) for x in hd.split("\t")[1:] if ":" in x)
+    tc = f.get("SO") == "unsorted" and f.get("GO") == "query" and ("SS" not in f or
+                                                                    f["SS"].rsplit(":", 1)[-1] == "template-coordinate")
+    if not (tc or (allow_unmapped and f.get("SO") == "queryname")):
+        raise ValueError("input BAM must be template-coordinate sorted" +
+                         (" or queryname sorted when unmapped reads are allowed" if allow_unmapped else ""))
+
+
+def mapped_bam_header(text: bytes) -> bytes:
+    """The binary BAM header of `text` with its reference list taken from the @SQ lines (SAM spec 4.2)."""
+    import struct
+    out = [b"BAM\1", struct.pack("<i", len(text)), text]
+    sq = []
+    for ln in text.split(b"\n"):
+        if ln.startswith(b"@SQ"):
+            f = dict(x.split(b":", 1) for x in ln.split(b"\t")[1:] if b":" in x)
+            sq.append((f[b"SN"], int(f[b"LN"])))
+    out.append(struct.pack("<i", len(sq)))
+    for nm, ln in sq:
+        out.append(struct.pack("<i", len(nm) + 1) + nm + b"\0" + struct.pack("<i", ln))
+    return b"".join(out)
+
+
+def group_records(text: bytes, bodies: np.ndarray, rec_off: np.ndarray, grouper, cell_tag: bytes = b"CB") -> bytes:
+    """`fgumi group` on a record stream in memory: position grouping, then the grouper; the MI-tagged stream
+    ([u32 block_size][record]...)."""
+    from .group import compact, group_by_position
+    keep, groups = group_by_position(bodies, rec_off, text, cell_tag)
+    bodies, rec_off = compact(bodies, rec_off, keep)
+    grouper.add_groups(bodies, rec_off, groups)
+    return grouper.flush()
+
+
+def group_file(in_path: str, out_path: str, grouper, n_threads: int = 4, level: int = 1,
+               cell_tag: bytes = b"CB") -> Dict[str, float]:
+    """`fgumi group -i mapped.bam -o grouped.bam` with an existing ReadGrouper (its options decide the rest)."""
+    lib = _l.load()
+    text, bodies, rec_off, tm = read_bam(in_path, n_threads)
+    check_group_sort_order(text, grouper.opt.umi.rules == _l.FGB_UMI_RULES_UNMAPPED)
+    t0 = time.perf_counter()
+    stream = group_records(text, bodies, rec_off, grouper, cell_tag)
+    t1 = time.perf_counter()
+    payload = mapped_bam_header(group_header(text)) + stream
+    cap = lib.fgb_bgzf_bound(len(payload))
+    comp = np.empty(cap, dtype=np.uint8)
+    cn = C.c_size_t()
+    st = lib.fgb_bgzf_compress(payload, len(payload), level, n_threads, 1, comp.ctypes.data, cap, C.addressof(cn))
+    if st != 0:
+        raise _l.FgbError(st, "fgb_bgzf_compress")
+    comp[:cn.value].tofile(out_path)
+    tm.update({"group_s": t1 - t0, "input_records": float(len(rec_off) - 1), "output_bytes": float(len(payload))})
+    return tm
+
+
+def split_stream(stream: bytes) -> Tuple[np.ndarray, np.ndarray]:
+    """[u32 block_size][record]... -> (record bodies back to back, rec_off) through fgb_bam_split_records."""
+    lib = _l.load()
+    buf = np.frombuffer(stream, np.uint8).copy() if stream else np.zeros(1, np.uint8)
+    cap = max(1, len(stream) // 36)
+    rec_off = np.zeros(cap + 1, np.uint64)
+    n, used = C.c_uint64(), C.c_size_t()
+    st = lib.fgb_bam_split_records(buf.ctypes.data, len(stream), buf.ctypes.data, rec_off.ctypes.data, cap,
+                                   C.addressof(n), C.addressof(used))
+    if st != 0:
+        raise _l.FgbError(st, "fgb_bam_split_records")
+    if used.value != len(stream):
+        raise ValueError("truncated record stream")
+    return buf[:int(rec_off[n.value])], rec_off[:n.value + 1]
+
+
+def group_and_call(in_path: str, grouper, caller, n_threads: int = 4, cell_tag: bytes = b"CB"):
+    """Mapped BAM -> `group` -> `simplex` or `duplex`, in memory: the grouper's MI-tagged stream goes through the MI
+    grouping (fgb_host_group_by_mi; the base MI for a DuplexConsensusCaller) into the caller, whose ConsensusOutput
+    is returned.  Records the grouper left without an MI (templates without a molecule) are not passed on, as the MI
+    grouping of `simplex` / `duplex` skips them."""
+    from .caller import ConsensusOutput, DuplexConsensusCaller
+    from .group import compact
+    lib = _l.load()
+    text, bodies, rec_off, _ = read_bam(in_path, n_threads)
+    check_group_sort_order(text, grouper.opt.umi.rules == _l.FGB_UMI_RULES_UNMAPPED)
+    gb, goff = split_stream(group_records(text, bodies, rec_off, grouper, cell_tag))
+    n = len(goff) - 1
+    keep = np.zeros(max(n, 1), np.uint8)
+    begin = np.zeros(n + 2, np.uint64)
+    ng = C.c_uint64()
+    st = lib.fgb_host_group_by_mi(gb.ctypes.data, goff.ctypes.data, n, bytes(grouper.opt.assign_tag),
+                                  int(isinstance(caller, DuplexConsensusCaller)), None, keep.ctypes.data,
+                                  begin.ctypes.data, C.addressof(ng))
+    if st != 0:
+        raise _l.FgbError(st, "fgb_host_group_by_mi")
+    gb, goff = compact(gb, goff, keep[:n])
+    st = lib.fgb_caller_add_groups(caller._h, gb.ctypes.data, goff.ctypes.data, begin.ctypes.data, ng.value)
+    caller._check(st, "fgb_caller_add_groups")
+    data, ln, cnt = C.c_void_p(), C.c_uint64(), C.c_uint64()
+    caller._check(lib.fgb_caller_flush(caller._h, C.byref(data), C.byref(ln), C.byref(cnt)), "fgb_caller_flush")
+    return ConsensusOutput(C.string_at(data.value, ln.value) if ln.value else b"", cnt.value)

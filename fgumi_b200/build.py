@@ -8,7 +8,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libfgumi_b200.so")
-SOURCES = ["capi.cu", "host_tables.cpp", "host/caller_host.cpp", "host/bgzf.cpp", "host/umi_host.cpp"]
+SOURCES = ["capi.cu", "host_tables.cpp", "host/caller_host.cpp", "host/bgzf.cpp", "host/umi_host.cpp",
+           "host/group_host.cpp"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-maxrregcount=112",      # upper bound only; vote_kernel must land at <= 96 (see _check_vote_kernel)

@@ -2696,6 +2696,8 @@ uint32_t fgb_struct_size(uint32_t id) {
     case 7: return sizeof(fgb_params);
     case 8: return sizeof(fgb_duplex_filter_params);
     case 9: return sizeof(fgb_record_columns);
+    case 10: return sizeof(fgb_umi_options);
+    case 11: return sizeof(fgb_group_options);
     default: return 0;
   }
 }

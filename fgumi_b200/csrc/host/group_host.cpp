@@ -1,0 +1,743 @@
+// `fgumi group` around the UMI assignment: position grouping of the input stream (fgb_host_group_by_position) and
+// the record-level grouper (fgb_grouper_*): templates, filter, orientation split and UMIs before fgb_umi_assign,
+// MI tags, order, histograms and the MI counter after it.  Restated in oracle/group_oracle.py, which cites the
+// reference (fgumi 0.2.0) line by line; the citations here are the same.
+#include <algorithm>
+#include <chrono>
+#include <cstring>
+#include <map>
+#include <memory>
+#include <new>
+#include <numeric>
+#include <string>
+#include <string_view>
+#include <tuple>
+#include <vector>
+
+#include "../../../include/fgumi_b200.h"
+#include "bam.h"
+#include "umi_host.h"
+
+namespace {
+
+using fgb::bam::View;
+namespace bam = fgb::bam;
+
+constexpr uint64_t kNone = UINT64_MAX;
+
+std::string_view read_name(const View& v) {
+  const uint32_t l = v.l_read_name();
+  return std::string_view(reinterpret_cast<const char*>(v.b + 32), l ? l - 1 : 0);
+}
+
+bool record_ok(const uint8_t* records, const uint64_t* rec_off, uint64_t i) {
+  if (rec_off[i + 1] < rec_off[i] || rec_off[i + 1] - rec_off[i] < 32) return false;
+  const View v(records + rec_off[i], rec_off[i + 1] - rec_off[i]);
+  return 32 + static_cast<size_t>(v.l_read_name()) <= v.n && v.cigar_in_bounds() && v.aux_off() <= v.n;
+}
+
+// tag_value_size (fields.rs:289-310); 0 = unknown type or truncated
+size_t tag_value_size(uint8_t t, const uint8_t* d, size_t n) {
+  switch (t) {
+    case 'A': case 'c': case 'C': return 1;
+    case 's': case 'S': return 2;
+    case 'i': case 'I': case 'f': return 4;
+    case 'Z': case 'H': {
+      const void* z = std::memchr(d, 0, n);
+      return z ? static_cast<const uint8_t*>(z) - d + 1 : 0;
+    }
+    case 'B': {
+      if (n < 5) return 0;
+      const uint8_t e = d[0];
+      const size_t es = (e == 'c' || e == 'C') ? 1 : (e == 's' || e == 'S') ? 2 : (e == 'i' || e == 'I' || e == 'f') ? 4 : 0;
+      return es ? 5 + static_cast<size_t>(bam::rd32(d + 1)) * es : 0;
+    }
+    default: return 0;
+  }
+}
+
+// unclipped_5prime_from_raw_bam (cigar.rs:201-228, 470-508): 1-based; 0 for an unmapped read, i32::MAX without CIGAR
+int32_t unclipped_5prime(const View& v) {
+  const uint16_t f = v.flags();
+  if (f & bam::kUnmapped) return 0;
+  const uint32_t n = v.n_cigar();
+  if (n == 0 || !v.cigar_in_bounds()) return INT32_MAX;
+  const int32_t pos = v.pos() + 1;
+  if (!(f & bam::kReverse)) {
+    int32_t clipped = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+      const uint32_t op = v.cigar_op(i);
+      if ((op & 0xF) == 4 || (op & 0xF) == 5) clipped += static_cast<int32_t>(op >> 4);
+      else break;
+    }
+    return pos - clipped;
+  }
+  int32_t ref_len = 0, trailing = 0;
+  bool saw = false;
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t op = v.cigar_op(i);
+    if (bam::consumes_ref(op & 0xF)) { ref_len += static_cast<int32_t>(op >> 4); trailing = 0; saw = true; }
+    else if (((op & 0xF) == 4 || (op & 0xF) == 5) && saw) trailing += static_cast<int32_t>(op >> 4);
+  }
+  return pos + ref_len + trailing - 1;
+}
+
+// ---- position grouping (unified_pipeline/bam.rs:415-499, base.rs:1375-1436, grouper.rs:406-588) ----------------
+struct PosKey {
+  int32_t ref1, pos1, ref2, pos2;
+  uint8_t strand1, strand2;
+  uint16_t library;
+  bool has_cell;
+  std::string cell;   // the reference compares a hash of the bytes; equal bytes <=> equal hash barring collisions
+  bool operator==(const PosKey& o) const {
+    return ref1 == o.ref1 && pos1 == o.pos1 && strand1 == o.strand1 && ref2 == o.ref2 && pos2 == o.pos2 &&
+           strand2 == o.strand2 && library == o.library && has_cell == o.has_cell && cell == o.cell;
+  }
+};
+
+// LibraryIndex::from_header (read_info.rs:104-131): libraries numbered from 1 in order of first appearance over the
+// @RG lines, an RG without LB is library "unknown" = 0, as is an RG the header does not declare.
+std::map<std::string, uint16_t> library_index(std::string_view text) {
+  std::map<std::string, uint16_t> lib_of_name{{"unknown", 0}}, lib_of_rg;
+  size_t p = 0;
+  while (p < text.size()) {
+    size_t e = text.find('\n', p);
+    if (e == std::string_view::npos) e = text.size();
+    std::string_view line = text.substr(p, e - p);
+    if (!line.empty() && line.back() == '\r') line.remove_suffix(1);
+    p = e + 1;
+    if (line.substr(0, 4) != "@RG\t") continue;
+    std::string id, lb = "unknown";
+    bool has_id = false;
+    size_t q = 4;
+    while (q <= line.size()) {
+      size_t t = line.find('\t', q);
+      if (t == std::string_view::npos) t = line.size();
+      std::string_view f = line.substr(q, t - q);
+      if (f.substr(0, 3) == "ID:") { id = std::string(f.substr(3)); has_id = true; }
+      else if (f.substr(0, 3) == "LB:") lb = std::string(f.substr(3));
+      q = t + 1;
+    }
+    if (!has_id) continue;
+    auto it = lib_of_name.find(lb);
+    if (it == lib_of_name.end()) it = lib_of_name.emplace(lb, static_cast<uint16_t>(lib_of_name.size())).first;
+    lib_of_rg[id] = it->second;
+  }
+  return lib_of_rg;
+}
+
+}  // namespace
+
+// ---- the grouper -------------------------------------------------------------------------------------------------
+namespace {
+
+struct Tpl {                    // one template's primary reads in its group's byte copy (kNone: absent)
+  uint64_t r1 = kNone, r1_len = 0, r2 = kNone, r2_len = 0;
+  uint64_t name = 0, name_len = 0;
+};
+
+struct GroupPrep {              // one position group after the host rules in front of the assignment
+  std::vector<uint8_t> bytes;
+  std::vector<Tpl> tpls;        // templates that passed the filter, in input order
+  std::vector<uint32_t> order;  // templates in call order (the calls concatenated)
+  std::vector<uint32_t> call_end;
+  std::string umis;             // per `order` entry: its UMI as umi_for_read made it
+  std::vector<uint64_t> umi_end;
+  uint64_t filter[6] = {0, 0, 0, 0, 0, 0};
+  bool dropped = false;         // the reference's assignment returns an error: nothing but the filter counts
+};
+
+enum { F_TOTAL, F_ACCEPTED, F_NON_PF, F_POOR, F_NS, F_SHORT };
+
+}  // namespace
+
+struct fgb_grouper {
+  fgb_group_options opt{};
+  fgb_umi_options umi{};        // what goes to fgb_umi_assign (no_umi: identity, 0 edits)
+  fgb_handle* h = nullptr;
+  std::vector<GroupPrep> queue;
+  uint64_t stats[FGB_GROUP_NSTATS] = {};
+  std::map<uint64_t, uint64_t> family_sizes, group_sizes;
+  std::string last_error;
+  // the UMI batch of the queue (fgb_grouper_pending), built on demand
+  bool batch_ready = false;
+  std::vector<uint8_t> b_umis;
+  std::vector<uint64_t> b_umi_off, b_call_off, b_group_off, b_group_of;   // b_group_of: queue index per batch group
+  std::vector<uint8_t> out;
+  double timing[5] = {0, 0, 0, 0, 0};   // fgb_grouper_last_timing
+};
+
+namespace {
+
+// filter_template_raw (group.rs:113-262): counts are per primary READ of the template
+bool filter_template(const fgb_grouper& g, const View* r1, const View* r2, uint64_t* fc) {
+  const uint64_t n = (r1 != nullptr) + (r2 != nullptr);
+  fc[F_TOTAL] += n;
+  if (!r1 && !r2) { fc[F_POOR] += n; return false; }
+  const bool both_unmapped = (!r1 || (r1->flags() & bam::kUnmapped)) && (!r2 || (r2->flags() & bam::kUnmapped));
+  if (both_unmapped && g.opt.umi.rules != FGB_UMI_RULES_UNMAPPED) { fc[F_POOR] += n; return false; }
+  const View* reads[2] = {r1, r2};
+  for (const View* r : reads) {   // phase 1: flags and MAPQ
+    if (!r) continue;
+    const uint16_t f = r->flags();
+    if (!g.opt.include_non_pf && (f & 0x200)) { fc[F_NON_PF] += n; return false; }
+    if (!(f & bam::kUnmapped) && r->b[9] < g.opt.min_map_q) { fc[F_POOR] += n; return false; }
+  }
+  for (const View* r : reads) {   // phase 2: one aux walk for MQ and the UMI (:157-221)
+    if (!r) continue;
+    const bool check_mq = !(r->flags() & bam::kMateUnmapped), check_umi = !g.opt.no_umi;
+    const uint8_t* a = r->b + r->aux_off();
+    const size_t an = r->n - r->aux_off();
+    bool have_mq = false, have_umi = false;
+    int64_t mq = 0;
+    const uint8_t* umi = nullptr;
+    size_t umi_len = 0;
+    size_t p = 0;
+    while (p + 3 <= an) {
+      const uint8_t t0 = a[p], t1 = a[p + 1], vt = a[p + 2];
+      if (check_umi && t0 == static_cast<uint8_t>(g.opt.umi_tag[0]) && t1 == static_cast<uint8_t>(g.opt.umi_tag[1]) && vt == 'Z') {
+        const void* z = std::memchr(a + p + 3, 0, an - (p + 3));
+        if (!z) break;
+        umi = a + p + 3;
+        umi_len = static_cast<const uint8_t*>(z) - umi;
+        have_umi = true;
+        p += 3 + umi_len + 1;
+        if (!check_mq || have_mq) break;
+        continue;
+      }
+      if (check_mq && t0 == 'M' && t1 == 'Q') {   // any integer type; a float or string MQ is None
+        const uint8_t* d = a + p + 3;
+        const size_t left = an - (p + 3);
+        have_mq = true;
+        switch (vt) {
+          case 'C': if (left >= 1) mq = d[0]; else have_mq = false; break;
+          case 'c': if (left >= 1) mq = static_cast<int8_t>(d[0]); else have_mq = false; break;
+          case 'S': if (left >= 2) mq = bam::rd16(d); else have_mq = false; break;
+          case 's': if (left >= 2) mq = static_cast<int16_t>(bam::rd16(d)); else have_mq = false; break;
+          case 'I': if (left >= 4) mq = bam::rd32(d); else have_mq = false; break;
+          case 'i': if (left >= 4) mq = bam::rdi32(d); else have_mq = false; break;
+          default: have_mq = false;
+        }
+      }
+      const size_t size = tag_value_size(vt, a + p + 3, an - (p + 3));
+      if (!size) break;
+      p += 3 + size;
+      if ((!check_umi || have_umi) && (!check_mq || have_mq)) break;
+    }
+    if (check_mq && have_mq && static_cast<uint8_t>(mq) < g.opt.min_map_q) { fc[F_POOR] += n; return false; }   // `as u8`
+    if (g.opt.no_umi) continue;
+    if (!have_umi) { fc[F_POOR] += n; return false; }
+    size_t bases = 0;   // validate_umi (fgumi-umi lib.rs:323-333)
+    for (size_t i = 0; i < umi_len; ++i) {
+      const uint8_t c = umi[i];
+      if (c == 'N') { fc[F_NS] += n; return false; }
+      if (c == 'A' || c == 'C' || c == 'G' || c == 'T' || c == 'a' || c == 'c' || c == 'g' || c == 't') ++bases;
+    }
+    if (g.opt.umi.min_umi_length && bases < g.opt.umi.min_umi_length) { fc[F_SHORT] += n; return false; }
+  }
+  fc[F_ACCEPTED] += n;
+  return true;
+}
+
+// One position group: templates, filter, split, UMIs.  "" or the message of an error that fails the whole call.
+std::string prepare_group(const fgb_grouper& g, const uint8_t* records, const uint64_t* rec_off, uint64_t b,
+                          uint64_t e, GroupPrep* gp) {
+  // build_templates_from_records (grouper.rs:596-651) + Template::from_records (template.rs:159-273)
+  std::vector<View> views;
+  views.reserve(e - b);
+  for (uint64_t i = b; i < e; ++i) views.emplace_back(records + rec_off[i], rec_off[i + 1] - rec_off[i]);
+  uint64_t i = 0;
+  const uint64_t n = e - b;
+  while (i < n) {
+    uint64_t j = i + 1;
+    const std::string_view name = read_name(views[i]);
+    while (j < n && read_name(views[j]) == name) ++j;
+    int64_t r1 = -1, r2 = -1;
+    for (uint64_t k = i; k < j; ++k) {
+      const uint16_t f = views[k].flags();
+      const bool is_r1 = !(f & bam::kPaired) || (f & bam::kFirst);
+      if (f & (bam::kSecondary | bam::kSupplementary)) continue;
+      int64_t& slot = is_r1 ? r1 : r2;
+      if (slot >= 0)
+        return std::string("Multiple non-secondary, non-supplemental ") + (is_r1 ? "R1" : "R2") + " records for read '" +
+               std::string(name) + "'";
+      slot = static_cast<int64_t>(k);
+    }
+    const View* v1 = r1 >= 0 ? &views[r1] : nullptr;
+    const View* v2 = r2 >= 0 ? &views[r2] : nullptr;
+    if (filter_template(g, v1, v2, gp->filter)) {
+      Tpl t;
+      auto copy = [&](const View* v, uint64_t* off, uint64_t* len) {
+        *off = gp->bytes.size();
+        *len = v->n;
+        gp->bytes.insert(gp->bytes.end(), v->b, v->b + v->n);
+      };
+      if (v1) copy(v1, &t.r1, &t.r1_len);
+      if (v2) copy(v2, &t.r2, &t.r2_len);
+      const uint64_t at = t.r1 != kNone ? t.r1 : t.r2;
+      t.name = at + 32;
+      t.name_len = name.size();
+      gp->tpls.push_back(t);
+    }
+    i = j;
+  }
+  if (gp->tpls.empty()) return "";
+  // the orientation split (group.rs:373-422): sub-groups in (r1_positive, r2_positive) order, false first; paired
+  // strategies take the whole group as one call
+  const size_t nt = gp->tpls.size();
+  auto view_of = [&](uint64_t off, uint64_t len) { return View(gp->bytes.data() + off, len); };
+  if (g.umi.strategy != FGB_UMI_PAIRED) {
+    std::vector<uint8_t> ori(nt);
+    for (size_t t = 0; t < nt; ++t) {
+      const Tpl& x = gp->tpls[t];
+      const bool p1 = x.r1 == kNone || !(view_of(x.r1, x.r1_len).flags() & bam::kReverse);
+      const bool p2 = x.r2 == kNone || !(view_of(x.r2, x.r2_len).flags() & bam::kReverse);
+      ori[t] = static_cast<uint8_t>(p1 * 2 + p2);
+    }
+    for (uint8_t o = 0; o < 4; ++o) {
+      const size_t before = gp->order.size();
+      for (size_t t = 0; t < nt; ++t) if (ori[t] == o) gp->order.push_back(static_cast<uint32_t>(t));
+      if (gp->order.size() > before) gp->call_end.push_back(static_cast<uint32_t>(gp->order.size()));
+    }
+  } else {
+    gp->order.resize(nt);
+    std::iota(gp->order.begin(), gp->order.end(), 0u);
+    gp->call_end.push_back(static_cast<uint32_t>(nt));
+  }
+  // the UMI of each template (group.rs:440-477): R1's tag if R1 exists, else R2's; umi_for_read on it
+  gp->umi_end.reserve(nt);
+  std::vector<uint8_t> buf;
+  for (uint32_t t : gp->order) {
+    if (!g.opt.no_umi) {
+      const Tpl& x = gp->tpls[t];
+      const View v = x.r1 != kNone ? view_of(x.r1, x.r1_len) : view_of(x.r2, x.r2_len);
+      const uint8_t* val = nullptr;
+      size_t len = 0;
+      if (!bam::find_string_tag(v, g.opt.umi_tag, &val, &len)) {   // "Missing UMI tag": the group is dropped
+        gp->dropped = true;
+        return "";
+      }
+      if (!bam::valid_utf8(val, len)) { gp->dropped = true; return ""; }   // "Invalid UTF-8 in UMI"
+      bool r1_earlier = true;   // is_r1_genomically_earlier_raw (:268-279)
+      if (x.r1 != kNone && x.r2 != kNone) {
+        const View a = view_of(x.r1, x.r1_len), c = view_of(x.r2, x.r2_len);
+        r1_earlier = a.ref_id() != c.ref_id() ? a.ref_id() < c.ref_id() : unclipped_5prime(a) <= unclipped_5prime(c);
+      }
+      buf.resize(2 * len + 2 * g.umi.edits + 16);
+      size_t out_len = 0;
+      if (fgb_host_umi_for_read(&g.umi, val, len, r1_earlier, buf.data(), buf.size(), &out_len) != FGB_OK) {
+        gp->dropped = true;   // a paired UMI that is not two parts around one '-' (:311-317)
+        return "";
+      }
+      gp->umis.append(reinterpret_cast<const char*>(buf.data()), out_len);
+    }
+    gp->umi_end.push_back(gp->umis.size());   // no_umi: every UMI is "" (:446-448)
+  }
+  return "";
+}
+
+// update_string_tag (fgumi-raw-bam tags.rs:694-721) on a copy of `rec`, appended to `out`: the first entry of the
+// tag (of any type) has its value overwritten when the lengths agree (its type byte is kept), is replaced by a Z
+// entry when they differ; a record without the tag gets one appended.
+void emit_with_tag(const uint8_t* rec, size_t n, const char tag[2], std::string_view val, std::vector<uint8_t>* out) {
+  const View v(rec, n);
+  const size_t aux = v.aux_off();
+  size_t p = aux, start = kNone, end = 0;
+  while (aux < n && p + 3 <= n) {
+    const size_t size = tag_value_size(rec[p + 2], rec + p + 3, n - (p + 3));
+    if (rec[p] == static_cast<uint8_t>(tag[0]) && rec[p + 1] == static_cast<uint8_t>(tag[1])) {
+      if (size) { start = p; end = p + 3 + size; }
+      break;
+    }
+    if (!size) break;
+    p += 3 + size;
+  }
+  const uint32_t bs0 = 0;
+  const size_t at = out->size();
+  out->insert(out->end(), reinterpret_cast<const uint8_t*>(&bs0), reinterpret_cast<const uint8_t*>(&bs0) + 4);
+  const uint8_t* vb = reinterpret_cast<const uint8_t*>(val.data());
+  const uint8_t z[3] = {static_cast<uint8_t>(tag[0]), static_cast<uint8_t>(tag[1]), 'Z'};
+  if (start != kNone && end - start - 4 == val.size()) {
+    out->insert(out->end(), rec, rec + n);
+    std::memcpy(out->data() + at + 4 + start + 3, vb, val.size());
+  } else if (start != kNone) {
+    out->insert(out->end(), rec, rec + start);
+    out->insert(out->end(), z, z + 3);
+    out->insert(out->end(), vb, vb + val.size());
+    out->push_back(0);
+    out->insert(out->end(), rec + end, rec + n);
+  } else {
+    out->insert(out->end(), rec, rec + n);
+    out->insert(out->end(), z, z + 3);
+    out->insert(out->end(), vb, vb + val.size());
+    out->push_back(0);
+  }
+  const uint32_t bs = static_cast<uint32_t>(out->size() - at - 4);
+  std::memcpy(out->data() + at, &bs, 4);
+}
+
+void emit_plain(const uint8_t* rec, size_t n, std::vector<uint8_t>* out) {
+  const uint32_t bs = static_cast<uint32_t>(n);
+  out->insert(out->end(), reinterpret_cast<const uint8_t*>(&bs), reinterpret_cast<const uint8_t*>(&bs) + 4);
+  out->insert(out->end(), rec, rec + n);
+}
+
+void build_batch(fgb_grouper* g) {
+  if (g->batch_ready) return;
+  g->b_umis.clear(); g->b_umi_off.assign(1, 0); g->b_call_off.assign(1, 0); g->b_group_off.assign(1, 0);
+  g->b_group_of.clear();
+  for (uint64_t q = 0; q < g->queue.size(); ++q) {
+    const GroupPrep& gp = g->queue[q];
+    if (gp.dropped || gp.tpls.empty()) continue;
+    const uint64_t base = g->b_umis.size();
+    g->b_umis.insert(g->b_umis.end(), gp.umis.begin(), gp.umis.end());
+    for (uint64_t e : gp.umi_end) g->b_umi_off.push_back(base + e);
+    const uint64_t ub = g->b_call_off.back();
+    for (uint32_t e : gp.call_end) g->b_call_off.push_back(ub + e);
+    g->b_group_off.push_back(g->b_call_off.size() - 1);
+    g->b_group_of.push_back(q);
+  }
+  g->batch_ready = true;
+}
+
+struct GroupOut {
+  std::vector<uint8_t> bytes;
+  std::vector<uint64_t> families;   // template count of each molecule, in output order
+  uint64_t n_records = 0;
+};
+
+// process_and_write_position_group after the assignment (group.rs:1524-1592, 1650-1682) for batch group `bg`.
+void emit_group(const fgb_grouper& g, const GroupPrep& gp, const uint64_t* ids, const uint8_t* kinds, uint64_t base_mi,
+                GroupOut* go) {
+  const size_t nt = gp.tpls.size();
+  std::vector<uint64_t> tid(nt), vidx(nt);   // vidx: MoleculeId::to_vec_index + 1, 0 = None (sorts first)
+  std::vector<uint8_t> tkind(nt);
+  for (size_t u = 0; u < nt; ++u) {
+    const uint32_t t = gp.order[u];
+    tkind[t] = kinds[u];
+    tid[t] = ids[u];
+    vidx[t] = kinds[u] == FGB_MOL_NONE ? 0
+            : kinds[u] == FGB_MOL_SINGLE ? ids[u] + 1
+            : 2 * ids[u] + (kinds[u] == FGB_MOL_B) + 1;
+  }
+  auto name = [&](size_t t) {
+    return std::string_view(reinterpret_cast<const char*>(gp.bytes.data() + gp.tpls[t].name), gp.tpls[t].name_len);
+  };
+  std::vector<uint32_t> sorted(nt);
+  std::iota(sorted.begin(), sorted.end(), 0u);
+  std::stable_sort(sorted.begin(), sorted.end(), [&](uint32_t a, uint32_t b) {
+    return vidx[a] != vidx[b] ? vidx[a] < vidx[b] : name(a) < name(b);
+  });
+  for (size_t s = 0; s < nt;) {   // family sizes (:1531-1560)
+    size_t e = s + 1;
+    while (e < nt && vidx[sorted[e]] == vidx[sorted[s]]) ++e;
+    if (vidx[sorted[s]]) go->families.push_back(e - s);
+    s = e;
+  }
+  std::string mi;
+  for (uint32_t t : sorted) {
+    const Tpl& x = gp.tpls[t];
+    const bool has = tkind[t] != FGB_MOL_NONE;
+    if (has) {
+      mi = std::to_string(tid[t] + base_mi);
+      if (tkind[t] == FGB_MOL_A) mi += "/A";
+      else if (tkind[t] == FGB_MOL_B) mi += "/B";
+    }
+    for (auto [off, len] : {std::pair<uint64_t, uint64_t>{x.r1, x.r1_len}, {x.r2, x.r2_len}}) {
+      if (off == kNone) continue;
+      if (has) emit_with_tag(gp.bytes.data() + off, len, g.opt.assign_tag, mi, &go->bytes);
+      else emit_plain(gp.bytes.data() + off, len, &go->bytes);
+      go->n_records++;
+    }
+  }
+}
+
+fgb_status finish_flush(fgb_grouper* g, const uint64_t* ids, const uint8_t* kinds, const uint64_t* mi_count,
+                        const uint8_t** out, uint64_t* out_len, uint64_t* n_records) {
+  const uint64_t ng = g->b_group_of.size();
+  std::vector<uint64_t> base(ng);
+  uint64_t next = g->stats[FGB_GSTAT_NEXT_MI];
+  for (uint64_t b = 0; b < ng; ++b) {   // the MI counter advances by max(id) + 1 per group (:1569-1575)
+    base[b] = next;
+    if (next + mi_count[b] < next) { g->last_error = "fgb_grouper_flush: MI counter overflow"; return FGB_ERR_INVALID_ARG; }
+    next += mi_count[b];
+  }
+  std::vector<GroupOut> outs(ng);
+  fgb_umi::parallel_for(ng, g->opt.umi.n_threads, [&](uint64_t b) {
+    const uint64_t u0 = g->b_call_off[g->b_group_off[b]];
+    emit_group(*g, g->queue[g->b_group_of[b]], ids + u0, kinds + u0, base[b], &outs[b]);
+  });
+  std::vector<uint64_t> at(ng + 1, 0);
+  uint64_t recs = 0;
+  for (uint64_t b = 0; b < ng; ++b) { at[b + 1] = at[b] + outs[b].bytes.size(); recs += outs[b].n_records; }
+  g->out.resize(at[ng]);
+  fgb_umi::parallel_for(ng, g->opt.umi.n_threads, [&](uint64_t b) {
+    if (!outs[b].bytes.empty()) std::memcpy(g->out.data() + at[b], outs[b].bytes.data(), outs[b].bytes.size());
+  });
+  for (uint64_t b = 0; b < ng; ++b) {
+    for (uint64_t f : outs[b].families) g->family_sizes[f]++;
+    if (!outs[b].families.empty()) g->group_sizes[outs[b].families.size()]++;
+  }
+  g->stats[FGB_GSTAT_NEXT_MI] = next;
+  g->stats[FGB_GSTAT_RECORDS_OUT] += recs;
+  g->queue.clear();
+  g->batch_ready = false;
+  *out = g->out.data();
+  *out_len = g->out.size();
+  *n_records = recs;
+  return FGB_OK;
+}
+
+template <class F>
+fgb_status guard(fgb_grouper* g, const char* where, F&& f) {
+  try {
+    return f();
+  } catch (const std::bad_alloc&) {
+    g->last_error = std::string(where) + ": out of host memory";
+  } catch (const std::exception& e) {
+    g->last_error = std::string(where) + ": " + e.what();
+  }
+  return FGB_ERR_NOMEM;
+}
+
+}  // namespace
+
+extern "C" {
+
+fgb_status fgb_host_group_by_position(const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
+                                      const char* header_text, size_t header_len, const char* cell_tag,
+                                      uint8_t* keep, uint64_t* group_begin, uint64_t* n_groups, uint64_t* bad_record) {
+  if (!keep || !group_begin || !n_groups || (n_records && (!records || !rec_off)) || (header_len && !header_text))
+    return FGB_ERR_INVALID_ARG;
+  if (bad_record) *bad_record = kNone;
+  try {
+    const auto libs = library_index(std::string_view(header_text ? header_text : "", header_len));
+    const char want[3][2] = {{'R', 'G'}, {'M', 'C'}, {cell_tag ? cell_tag[0] : '\0', cell_tag ? cell_tag[1] : '\0'}};
+    PosKey cur{};
+    bool have = false;
+    uint64_t kept = 0, groups = 0, last = 0;
+    for (uint64_t i = 0; i < n_records; ++i) {
+      if (!record_ok(records, rec_off, i)) { if (bad_record) *bad_record = i; return FGB_ERR_LAYOUT; }
+      const View v(records + rec_off[i], rec_off[i + 1] - rec_off[i]);
+      const uint16_t f = v.flags();
+      keep[i] = 0;
+      if (f & (bam::kSecondary | bam::kSupplementary)) continue;   // grouper.rs:489-493
+      const uint8_t* val[3];
+      size_t len[3];
+      bam::find_string_tags(v, want, cell_tag ? 3 : 2, val, len);
+      const bool mc = val[1] && bam::valid_utf8(val[1], len[1]);
+      const bool paired = f & bam::kPaired, mate_unmapped = f & bam::kMateUnmapped;
+      if (paired && !(f & bam::kUnmapped) && !mate_unmapped && !mc) {   // validate_mc_tag (:452-475)
+        if (bad_record) *bad_record = i;
+        return FGB_ERR_INVALID_ARG;
+      }
+      PosKey k{};
+      k.library = 0;
+      if (val[0]) {
+        auto it = libs.find(std::string(reinterpret_cast<const char*>(val[0]), len[0]));
+        if (it != libs.end()) k.library = it->second;
+      }
+      k.has_cell = cell_tag && val[2];
+      if (k.has_cell) k.cell.assign(reinterpret_cast<const char*>(val[2]), len[2]);
+      const int32_t own_ref = v.ref_id(), own_pos = unclipped_5prime(v);
+      const uint8_t strand = (f & bam::kReverse) ? 1 : 0;
+      k.ref1 = own_ref; k.pos1 = own_pos; k.strand1 = strand;
+      k.ref2 = INT32_MAX; k.pos2 = INT32_MAX; k.strand2 = UINT8_MAX;
+      if (paired && !mate_unmapped && mc) {   // GroupKey::paired, lower (ref, pos, strand) first
+        const char* c = reinterpret_cast<const char*>(val[1]);
+        const bool mrev = f & bam::kMateReverse;
+        const int32_t mpos1 = v.mate_pos() + 1;
+        int32_t mp;
+        if (mrev) {
+          int32_t rl, tr;
+          bam::mc_ref_len_and_trailing(c, len[1], &rl, &tr);
+          mp = mpos1 + rl + tr - 1;
+        } else {
+          mp = mpos1 - bam::mc_leading_clips(c, len[1]);
+        }
+        const uint8_t ms = mrev ? 1 : 0;
+        const int32_t mref = v.mate_ref_id();
+        if (std::make_tuple(own_ref, own_pos, strand) <= std::make_tuple(mref, mp, ms)) {
+          k.ref2 = mref; k.pos2 = mp; k.strand2 = ms;
+        } else {
+          k.ref1 = mref; k.pos1 = mp; k.strand1 = ms;
+          k.ref2 = own_ref; k.pos2 = own_pos; k.strand2 = strand;
+        }
+      }
+      keep[i] = 1;
+      bool same = have && k == cur;
+      if (have && !same) {   // a new position continuing the previous record's QNAME stays (unmapped mates)
+        const View lv(records + rec_off[last], rec_off[last + 1] - rec_off[last]);
+        same = read_name(lv) == read_name(v);
+      }
+      if (!same) { group_begin[groups++] = kept; cur = std::move(k); have = true; }
+      last = i;
+      ++kept;
+    }
+    group_begin[groups] = kept;
+    *n_groups = groups;
+  } catch (const std::bad_alloc&) {
+    return FGB_ERR_NOMEM;
+  }
+  return FGB_OK;
+}
+
+fgb_status fgb_grouper_create(int device, const fgb_group_options* opt, fgb_grouper** out) {
+  if (!opt || !out) return FGB_ERR_INVALID_ARG;
+  *out = nullptr;
+  fgb_umi_options u = opt->umi;
+  if (opt->no_umi) { u.strategy = FGB_UMI_IDENTITY; u.edits = 0; u.min_umi_length = 0; }   // group.rs:732-757
+  if (!fgb_umi::check_options(u).empty()) return FGB_ERR_INVALID_ARG;
+  if (opt->umi.strategy == FGB_UMI_PAIRED && (opt->umi.min_umi_length || opt->no_umi)) return FGB_ERR_INVALID_ARG;   // :723-730
+  std::unique_ptr<fgb_grouper> g(new (std::nothrow) fgb_grouper());
+  if (!g) return FGB_ERR_NOMEM;
+  g->opt = *opt;
+  g->umi = u;
+  g->stats[FGB_GSTAT_NEXT_MI] = opt->first_mi;
+  if (device != FGB_DEVICE_NONE) {
+    fgb_params p{};
+    p.error_rate_pre_umi = 45;
+    p.error_rate_post_umi = 40;
+    p.min_consensus_base_quality = 40;
+    p.min_reads = 1;
+    const fgb_status st = fgb_create(device, &p, &g->h);
+    if (st != FGB_OK) return st;
+  }
+  *out = g.release();
+  return FGB_OK;
+}
+
+void fgb_grouper_destroy(fgb_grouper* g) {
+  if (!g) return;
+  if (g->h) fgb_destroy(g->h);
+  delete g;
+}
+
+size_t fgb_grouper_last_error(const fgb_grouper* g, char* buf, size_t buf_len) {
+  if (!g) return 0;
+  if (buf && buf_len) {
+    const size_t n = std::min(buf_len - 1, g->last_error.size());
+    std::memcpy(buf, g->last_error.data(), n);
+    buf[n] = 0;
+  }
+  return g->last_error.size();
+}
+
+fgb_status fgb_grouper_add_groups(fgb_grouper* g, const uint8_t* records, const uint64_t* rec_off,
+                                  const uint64_t* group_rec, uint64_t n_groups) {
+  if (!g || !group_rec || (n_groups && (!records || !rec_off))) return FGB_ERR_INVALID_ARG;
+  return guard(g, "fgb_grouper_add_groups", [&]() -> fgb_status {
+    for (uint64_t x = 0; x < n_groups; ++x)
+      if (group_rec[x + 1] < group_rec[x]) { g->last_error = "fgb_grouper_add_groups: group_rec descends"; return FGB_ERR_LAYOUT; }
+    const uint64_t r0 = n_groups ? group_rec[0] : 0, r1 = n_groups ? group_rec[n_groups] : 0;
+    for (uint64_t i = r0; i < r1; ++i)
+      if (!record_ok(records, rec_off, i)) {
+        g->last_error = "fgb_grouper_add_groups: record " + std::to_string(i) + " is malformed";
+        return FGB_ERR_LAYOUT;
+      }
+    std::vector<GroupPrep> prep(n_groups);
+    std::vector<std::string> err(n_groups);
+    fgb_umi::parallel_for(n_groups, g->opt.umi.n_threads, [&](uint64_t x) {
+      err[x] = prepare_group(*g, records, rec_off, group_rec[x], group_rec[x + 1], &prep[x]);
+    });
+    for (uint64_t x = 0; x < n_groups; ++x)
+      if (!err[x].empty()) {
+        g->last_error = "fgb_grouper_add_groups: position group " + std::to_string(x) + ": " + err[x];
+        return FGB_ERR_INVALID_ARG;
+      }
+    g->queue.reserve(g->queue.size() + n_groups);
+    for (auto& gp : prep) {
+      for (int k = 0; k < 6; ++k) g->stats[FGB_GSTAT_TOTAL + k] += gp.filter[k];
+      g->stats[FGB_GSTAT_POSITION_GROUPS]++;
+      if (gp.dropped) g->stats[FGB_GSTAT_GROUPS_DROPPED]++;
+      if (gp.dropped || gp.tpls.empty()) continue;   // nothing of it reaches the output
+      g->queue.push_back(std::move(gp));
+    }
+    g->batch_ready = false;
+    return FGB_OK;
+  });
+}
+
+fgb_status fgb_grouper_pending(fgb_grouper* g, const uint8_t** umis, const uint64_t** umi_off, uint64_t* n_umis,
+                               const uint64_t** call_off, uint64_t* n_calls, const uint64_t** group_off,
+                               uint64_t* n_groups) {
+  if (!g || !umis || !umi_off || !n_umis || !call_off || !n_calls || !group_off || !n_groups) return FGB_ERR_INVALID_ARG;
+  return guard(g, "fgb_grouper_pending", [&]() -> fgb_status {
+    build_batch(g);
+    *umis = g->b_umis.data();
+    *umi_off = g->b_umi_off.data();
+    *n_umis = g->b_umi_off.size() - 1;
+    *call_off = g->b_call_off.data();
+    *n_calls = g->b_call_off.size() - 1;
+    *group_off = g->b_group_off.data();
+    *n_groups = g->b_group_off.size() - 1;
+    return FGB_OK;
+  });
+}
+
+fgb_status fgb_grouper_flush(fgb_grouper* g, const uint8_t** out, uint64_t* out_len, uint64_t* n_records) {
+  if (!g || !out || !out_len || !n_records) return FGB_ERR_INVALID_ARG;
+  if (!g->h) { g->last_error = "fgb_grouper_flush: a planning-only grouper has no device"; return FGB_ERR_NO_DEVICE; }
+  return guard(g, "fgb_grouper_flush", [&]() -> fgb_status {
+    build_batch(g);
+    const uint64_t n = g->b_umi_off.size() - 1, nc = g->b_call_off.size() - 1, ng = g->b_group_off.size() - 1;
+    std::vector<uint64_t> ids(n + 1), counts(ng + 1);
+    std::vector<uint8_t> kinds(n + 1);
+    static const uint8_t kNoBytes = 0;   // every UMI empty (no_umi): the ABI still wants a pointer
+    const uint8_t* umis = g->b_umis.empty() ? &kNoBytes : g->b_umis.data();
+    const fgb_status st = fgb_umi_assign(g->h, &g->umi, umis, g->b_umi_off.data(), n,
+                                         g->b_call_off.data(), nc, g->b_group_off.data(), ng, ids.data(),
+                                         kinds.data(), counts.data());
+    if (st != FGB_OK) {
+      std::string e(fgb_last_error(g->h, nullptr, 0), '\0');
+      fgb_last_error(g->h, &e[0], e.size() + 1);
+      g->last_error = "fgb_grouper_flush: " + e;
+      return st;
+    }
+    fgb_umi_last_timing(g->h, g->timing);
+    const auto t0 = std::chrono::steady_clock::now();
+    const fgb_status fs = finish_flush(g, ids.data(), kinds.data(), counts.data(), out, out_len, n_records);
+    g->timing[4] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return fs;
+  });
+}
+
+fgb_status fgb_grouper_last_timing(const fgb_grouper* g, double ms[5]) {
+  if (!g || !ms) return FGB_ERR_INVALID_ARG;
+  std::memcpy(ms, g->timing, sizeof(g->timing));
+  return FGB_OK;
+}
+
+fgb_status fgb_grouper_flush_with_ids(fgb_grouper* g, const uint64_t* ids, const uint8_t* kinds,
+                                      const uint64_t* group_mi_count, const uint8_t** out, uint64_t* out_len,
+                                      uint64_t* n_records) {
+  if (!g || !out || !out_len || !n_records) return FGB_ERR_INVALID_ARG;
+  return guard(g, "fgb_grouper_flush_with_ids", [&]() -> fgb_status {
+    build_batch(g);
+    const uint64_t n = g->b_umi_off.size() - 1, ng = g->b_group_off.size() - 1;
+    if ((n && (!ids || !kinds)) || (ng && !group_mi_count)) return FGB_ERR_INVALID_ARG;
+    for (uint64_t u = 0; u < n; ++u)
+      if (kinds[u] > FGB_MOL_B) { g->last_error = "fgb_grouper_flush_with_ids: unknown kind"; return FGB_ERR_INVALID_ARG; }
+    return finish_flush(g, ids, kinds, group_mi_count, out, out_len, n_records);
+  });
+}
+
+fgb_status fgb_grouper_stats(const fgb_grouper* g, uint64_t stats[FGB_GROUP_NSTATS]) {
+  if (!g || !stats) return FGB_ERR_INVALID_ARG;
+  std::memcpy(stats, g->stats, sizeof(g->stats));
+  return FGB_OK;
+}
+
+fgb_status fgb_grouper_histogram(const fgb_grouper* g, int which, uint64_t* sizes, uint64_t* counts, uint64_t cap,
+                                 uint64_t* n) {
+  if (!g || !n || (which != FGB_GROUP_HIST_FAMILY && which != FGB_GROUP_HIST_POSITION)) return FGB_ERR_INVALID_ARG;
+  const auto& h = which == FGB_GROUP_HIST_FAMILY ? g->family_sizes : g->group_sizes;
+  *n = h.size();
+  if (cap < h.size()) return FGB_OK;
+  if (h.size() && (!sizes || !counts)) return FGB_ERR_INVALID_ARG;
+  uint64_t i = 0;
+  for (const auto& [s, c] : h) { sizes[i] = s; counts[i] = c; ++i; }
+  return FGB_OK;
+}
+
+}  // extern "C"

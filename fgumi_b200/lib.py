@@ -197,6 +197,19 @@ class FgbUmiOptions(C.Structure):
                 ("min_umi_length", C.c_uint32), ("n_threads", C.c_uint32), ("reserved", C.c_uint32)]
 
 
+class FgbGroupOptions(C.Structure):
+    _fields_ = [("umi", FgbUmiOptions), ("min_map_q", C.c_uint8), ("include_non_pf", C.c_uint8),
+                ("no_umi", C.c_uint8), ("reserved0", C.c_uint8), ("umi_tag", C.c_char * 2),
+                ("assign_tag", C.c_char * 2), ("first_mi", C.c_uint64)]
+
+
+FGB_GROUP_NSTATS = 12
+GROUP_STAT_NAMES = ("total_records", "accepted_records", "discarded_non_pf", "discarded_poor_alignment",
+                    "discarded_ns_in_umi", "discarded_umi_too_short", "position_groups", "groups_dropped", "next_mi",
+                    "records_out")
+FGB_GROUP_HIST_FAMILY, FGB_GROUP_HIST_POSITION = 0, 1
+
+
 class FgbUmiKey(C.Structure):
     _fields_ = [("bits", C.c_uint64), ("str_off", C.c_uint64), ("str_len", C.c_uint32), ("count", C.c_uint32),
                 ("first", C.c_uint32), ("dash", C.c_uint32), ("len", C.c_uint8), ("flags", C.c_uint8),
@@ -230,6 +243,9 @@ SYMBOLS = (
     "fgb_host_num_bases_extending_past_mate", "fgb_host_clip_cigar_ops", "fgb_host_read_pos_at_ref_pos", "fgb_host_simplify_cigar", "fgb_host_source_reads", "fgb_host_consensus_umis", "fgb_caller_pending", "fgb_host_simplex_record", "fgb_bgzf_bound", "fgb_bgzf_compress", "fgb_bgzf_scan_members", "fgb_bgzf_inflate_device", "fgb_host_inflate_member", "fgb_bam_header", "fgb_bgzf_uncompressed_size", "fgb_bgzf_decompress", "fgb_bam_read_header", "fgb_bam_split_records", "fgb_host_group_by_mi", "fgb_host_duplex_record",
     "fgb_umi_assign", "fgb_host_umi_for_read", "fgb_host_umi_prepare", "fgb_host_umi_resolve",
     "fgb_umi_edges", "fgb_umi_last_timing",
+    "fgb_host_group_by_position", "fgb_grouper_create", "fgb_grouper_destroy", "fgb_grouper_last_error",
+    "fgb_grouper_add_groups", "fgb_grouper_pending", "fgb_grouper_flush", "fgb_grouper_flush_with_ids",
+    "fgb_grouper_stats", "fgb_grouper_histogram", "fgb_grouper_last_timing",
 )
 
 _lib = None
@@ -411,6 +427,30 @@ def load() -> C.CDLL:
     lib.fgb_umi_edges.restype = C.c_int32
     lib.fgb_umi_last_timing.argtypes = [vp, vp]
     lib.fgb_umi_last_timing.restype = C.c_int32
+    lib.fgb_host_group_by_position.argtypes = [vp, vp, u64, C.c_char_p, C.c_size_t, C.c_char_p, vp, vp,
+                                               C.POINTER(u64), C.POINTER(u64)]
+    lib.fgb_host_group_by_position.restype = C.c_int32
+    lib.fgb_grouper_create.argtypes = [C.c_int, C.POINTER(FgbGroupOptions), C.POINTER(vp)]
+    lib.fgb_grouper_create.restype = C.c_int32
+    lib.fgb_grouper_destroy.argtypes = [vp]
+    lib.fgb_grouper_destroy.restype = None
+    lib.fgb_grouper_last_error.argtypes = [vp, C.c_char_p, C.c_size_t]
+    lib.fgb_grouper_last_error.restype = C.c_size_t
+    lib.fgb_grouper_add_groups.argtypes = [vp, vp, vp, vp, u64]
+    lib.fgb_grouper_add_groups.restype = C.c_int32
+    lib.fgb_grouper_pending.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(u64), C.POINTER(vp),
+                                        C.POINTER(u64), C.POINTER(vp), C.POINTER(u64)]
+    lib.fgb_grouper_pending.restype = C.c_int32
+    lib.fgb_grouper_flush.argtypes = [vp, C.POINTER(vp), C.POINTER(u64), C.POINTER(u64)]
+    lib.fgb_grouper_flush.restype = C.c_int32
+    lib.fgb_grouper_flush_with_ids.argtypes = [vp, vp, vp, vp, C.POINTER(vp), C.POINTER(u64), C.POINTER(u64)]
+    lib.fgb_grouper_flush_with_ids.restype = C.c_int32
+    lib.fgb_grouper_stats.argtypes = [vp, vp]
+    lib.fgb_grouper_stats.restype = C.c_int32
+    lib.fgb_grouper_histogram.argtypes = [vp, C.c_int, vp, vp, u64, C.POINTER(u64)]
+    lib.fgb_grouper_histogram.restype = C.c_int32
+    lib.fgb_grouper_last_timing.argtypes = [vp, vp]
+    lib.fgb_grouper_last_timing.restype = C.c_int32
     lib.fgb_struct_size.argtypes = [C.c_uint32]
     lib.fgb_struct_size.restype = C.c_uint32
     _lib = lib

@@ -272,3 +272,112 @@ def umi_families(n_molecules: int, length: int, mean_family: float = 4.0, error_
         swap = rng.random(len(out)) < swap_rate
         out = [(u[length:] + "-" + u[:length]) if s else (u[:length] + "-" + u[length:]) for u, s in zip(out, swap)]
     return out
+
+
+def mapped_templates(n_sites: int, molecules: int = 3, mean_family: float = 3.0, umi_length: int = 8,
+                     paired_umis: bool = False, umi_error_rate: float = 0.02, n_umi_rate: float = 0.0,
+                     no_dash_rate: float = 0.0, low_mapq_rate: float = 0.0, qc_fail_rate: float = 0.0,
+                     unmapped_mate_rate: float = 0.0, secondary_rate: float = 0.0, reverse_rate: float = 0.3,
+                     cross_contig_rate: float = 0.0, amplicon_molecules: int = 0, read_length: int = 20,
+                     seed: int = 0):
+    """Seeded template-coordinate-sorted mapped paired-end templates, as `fgumi group` takes them: (SAM header text,
+    record bodies uint8[...], rec_off uint64[n + 1]).
+
+    Each site is one position: `molecules` true UMIs (RX, "X-Y" with `paired_umis`, the halves swapped on the
+    templates of the other strand), family sizes 1 + Poisson(mean_family - 1), each UMI base substituted with
+    probability `umi_error_rate`.  Each molecule has its own R1 and R2 sequences, copied into its reads with 2 %
+    substitutions and qualities 20-40.  Records carry RX, MC, MQ, RG (three read groups, two sharing a library) and CB
+    (one cell per site).  Per template, with the given rates: an upper-case N in the UMI, a UMI without its '-',
+    MAPQ 0 on one read, the QC-fail flag, a supplementary and a secondary record after the primaries, and the pair
+    on the other contig.  With `unmapped_mate_rate` a site is followed by a site of templates whose R2 is unmapped.
+    `amplicon_molecules` > 0 adds one site with that many molecules (one large call)."""
+    import struct
+    rng = np.random.default_rng(seed)
+    header = ("@HD\tVN:1.6\tSO:unsorted\tGO:query\tSS:unsorted:template-coordinate\n"
+              "@SQ\tSN:chr1\tLN:100000000\n@SQ\tSN:chr2\tLN:100000000\n"
+              "@RG\tID:A\tSM:s\tLB:L1\n@RG\tID:B\tSM:s\tLB:L1\n@RG\tID:C\tSM:s\tLB:L2\n"
+              "@PG\tID:bwa\tPN:bwa\tCL:bwa mem\n").encode()
+    L = read_length
+    nib = np.array([1, 2, 4, 8], np.uint8)             # A C G T in BAM's 4-bit code
+    cig = struct.pack("<I", (L << 4) | 0)
+    mc = b"%dM" % L
+    out = []
+    tnum = 0
+
+    def read_bytes(true):
+        """Packed SEQ and QUAL of one read of a molecule: 2 % substitutions, qualities 20-40."""
+        b = np.where(rng.random(L) < 0.02, (true + rng.integers(1, 4, size=L)) % 4, true)
+        n = nib[b]
+        if L % 2:
+            n = np.concatenate([n, np.zeros(1, np.uint8)])
+        return ((n[0::2] << 4) | n[1::2]).tobytes() + rng.integers(20, 41, size=L, dtype=np.uint8).tobytes()
+
+    def rec(name, flag, ref, pos, mapq, mref, mpos, tags, true):
+        r = (struct.pack("<iiBBHHHIiii", ref, pos, len(name) + 1, mapq, 4680, 0 if flag & 4 else 1, flag, L, mref,
+                         mpos, 0) + name + b"\0" + (b"" if flag & 4 else cig) + read_bytes(true) + tags)
+        out.append(r)
+
+    def ztag(t, v):
+        return t + b"Z" + v + b"\0"
+
+    def umi_str(true, strand_b):
+        u = true.copy()
+        err = rng.random(len(u)) < umi_error_rate
+        u = np.where(err, (u + rng.integers(1, 4, size=len(u))) % 4, u)
+        s = bytearray(ACGT[u].tobytes())
+        if rng.random() < n_umi_rate:
+            s[int(rng.integers(0, len(s)))] = ord("N")
+        if paired_umis:
+            h = len(s) // 2
+            a, b = bytes(s[:h]), bytes(s[h:])
+            if strand_b:
+                a, b = b, a
+            return a + b + b"" if rng.random() < no_dash_rate else a + b"-" + b
+        return bytes(s)
+
+    def site(pos, n_mol, unmapped_mates):
+        nonlocal tnum
+        rg = [b"A", b"B", b"C"][int(rng.integers(0, 3))]
+        cb = b"CELL%d" % int(rng.integers(0, 4))
+        width = 2 * umi_length if paired_umis else umi_length
+        trues = rng.integers(0, 4, size=(n_mol, width))
+        bases = rng.integers(0, 4, size=(n_mol, 2, L))     # the molecule's R1 and R2 sequences
+        sizes = 1 + rng.poisson(max(mean_family - 1.0, 0.0), size=n_mol)
+        cross = (not unmapped_mates) and rng.random() < cross_contig_rate
+        for m in range(n_mol):
+            for _ in range(int(sizes[m])):
+                tnum += 1
+                name = b"t%09d" % tnum
+                rev = rng.random() < reverse_rate    # R1 reverse, R2 forward: the other strand of the molecule
+                u = umi_str(trues[m], rev)
+                q1 = 0 if rng.random() < low_mapq_rate else 60
+                qc = 0x200 if rng.random() < qc_fail_rate else 0
+                common = ztag(b"RX", u) + ztag(b"RG", rg) + ztag(b"CB", cb)
+                if unmapped_mates:
+                    rec(name, 0x1 | 0x8 | 0x40 | qc, 0, pos, q1, 0, pos, common, bases[m, 0])
+                    rec(name, 0x1 | 0x4 | 0x80, 0, pos, 0, 0, pos, common, bases[m, 1])
+                    continue
+                r2ref = 1 if cross else 0
+                r2pos = pos if cross else pos + 50
+                f1 = 0x1 | 0x2 | 0x40 | qc | (0x10 if rev else 0x20)
+                f2 = 0x1 | 0x2 | 0x80 | (0x20 if rev else 0x10)
+                mq = b"MQi" + struct.pack("<i", 60)
+                if rev:   # R1 on the reverse strand at the right end; R2 forward at the left
+                    p1, ref1, p2, ref2 = r2pos, r2ref, pos, 0
+                else:
+                    p1, ref1, p2, ref2 = pos, 0, r2pos, r2ref
+                rec(name, f1, ref1, p1, q1, ref2, p2, common + ztag(b"MC", mc) + mq, bases[m, 0])
+                rec(name, f2, ref2, p2, 60, ref1, p1, common + ztag(b"MC", mc) + b"MQi" + struct.pack("<i", q1), bases[m, 1])
+                if rng.random() < secondary_rate:
+                    rec(name, f1 | 0x800, ref1, p1 + 7, 60, ref2, p2, common, bases[m, 0])
+                    rec(name, f1 | 0x100, ref1, p1 + 9, 60, ref2, p2, common, bases[m, 0])
+
+    for s in range(n_sites):
+        site(1000 + 200 * s, molecules, False)
+        if rng.random() < unmapped_mate_rate:
+            site(1000 + 200 * s + 100, max(1, molecules // 2), True)
+    if amplicon_molecules:
+        site(1000 + 200 * n_sites + 500, amplicon_molecules, False)
+    off = np.zeros(len(out) + 1, np.uint64)
+    off[1:] = np.cumsum([len(r) for r in out])
+    return header, np.frombuffer(b"".join(out) or b"\0", np.uint8)[:int(off[-1])].copy(), off

@@ -899,10 +899,87 @@ fgb_status fgb_umi_edges(fgb_handle* h, const fgb_umi_options* opt, const uint8_
  * pass with its sort / scan and around the fill pass), [3] the rules and numbering on the host. */
 fgb_status fgb_umi_last_timing(const fgb_handle* h, double ms[4]);
 
+/* ---- `fgumi group` from raw records (src/lib/commands/group.rs, src/lib/grouper.rs; host code around fgb_umi_assign)
+ * Position grouping of an input stream (compute_group_key_from_raw, unified_pipeline/bam.rs:415-499, and
+ * RecordPositionGrouper, grouper.rs:406-588): secondary and supplementary records are skipped (keep[i] = 0); the
+ * others form groups of consecutive records with the same key -- both unclipped 5' ends (the mate's through MC), lower
+ * first, the library of the RG (RGs sharing an LB are one library, an unknown RG is library 0; `header_text` is the
+ * SAM header) and, when cell_tag is given, the cell barcode -- and a record at a new key whose QNAME continues the
+ * previous kept record's stays in its group (unmapped mates).  group_begin (room for n_records + 1 entries) indexes
+ * the KEPT records, the table fgb_grouper_add_groups takes once the skipped records are dropped.  A paired, mapped
+ * primary record with a mapped mate and no MC tag fails the call with FGB_ERR_INVALID_ARG and *bad_record = its index;
+ * a malformed record gives FGB_ERR_LAYOUT.  Library, cell and QNAME are compared as bytes where the reference
+ * compares their hashes (the same answer barring a hash collision). */
+fgb_status fgb_host_group_by_position(const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
+                                      const char* header_text, size_t header_len, const char* cell_tag,
+                                      uint8_t* keep, uint64_t* group_begin, uint64_t* n_groups, uint64_t* bad_record);
+
+typedef struct fgb_group_options {
+  fgb_umi_options umi;      /* strategy / edits / min_umi_length / n_threads; rules = FGB_UMI_RULES_UNMAPPED is
+                               --allow-unmapped (the parallel assigners AND the filter's both-unmapped rule)      */
+  uint8_t min_map_q;        /* 1 in the CLI                                                                      */
+  uint8_t include_non_pf;   /* 0 */
+  uint8_t no_umi;           /* group by position only: identity, 0 edits, every UMI "" (group.rs:732-757)        */
+  uint8_t reserved0;
+  char umi_tag[2];          /* "RX" */
+  char assign_tag[2];       /* "MI" */
+  uint64_t first_mi;        /* MI number of the first molecule                                                   */
+} fgb_group_options;
+
+enum {   /* fgb_grouper_stats: FilterMetrics (group.rs:113-262, per primary READ) and the grouper's own counters */
+  FGB_GSTAT_TOTAL = 0, FGB_GSTAT_ACCEPTED = 1, FGB_GSTAT_DISCARDED_NON_PF = 2, FGB_GSTAT_DISCARDED_POOR_ALIGNMENT = 3,
+  FGB_GSTAT_DISCARDED_NS_IN_UMI = 4, FGB_GSTAT_DISCARDED_UMI_TOO_SHORT = 5,
+  FGB_GSTAT_POSITION_GROUPS = 6,   /* position groups added                                                      */
+  FGB_GSTAT_GROUPS_DROPPED = 7,    /* position groups whose assignment the reference rejects (a paired UMI without
+                                      exactly one '-', a UMI that is not UTF-8): logged and skipped there          */
+  FGB_GSTAT_NEXT_MI = 8,           /* MI number of the next molecule                                             */
+  FGB_GSTAT_RECORDS_OUT = 9,
+  FGB_GROUP_NSTATS = 12
+};
+enum { FGB_GROUP_HIST_FAMILY = 0, FGB_GROUP_HIST_POSITION = 1 };
+
+/* The record-level grouper: process_and_write_position_group (group.rs:1460-1592) per position group.
+ * add_groups (group g = records [group_rec[g], group_rec[g+1]) of the rec_off table) runs, on n_threads host threads
+ * over contiguous ranges of groups: templates from consecutive records with one QNAME, filter_template_raw, the
+ * pair-orientation split (non-paired strategies; sub-groups in (r1+, r2+) order, false first), the UMI of R1 (else
+ * R2) through umi_for_read.  The records of templates that pass are copied; the caller's buffers are free again on
+ * return.  A template with two primary R1s (or R2s) or a malformed record fails the call (FGB_ERR_INVALID_ARG /
+ * FGB_ERR_LAYOUT) and leaves nothing of it queued; a group the reference would drop is counted and dropped.
+ * flush sends every queued group through fgb_umi_assign in one device phase (a mapped adjacency call with UMIs of
+ * different lengths fails it with FGB_ERR_INVALID_ARG and changes nothing), sorts each group's templates stably by
+ * (MoleculeId::to_vec_index, QNAME), None first, counts family and position-group sizes, and emits the primary records
+ * with the assign tag set (update_string_tag, tags.rs:694-721; a template without an ID unchanged), each with its
+ * block_size word, in input order and byte-identical for any n_threads.  *out stays valid until the next flush or
+ * destroy.  device == FGB_DEVICE_NONE: planning only -- flush fails with FGB_ERR_NO_DEVICE; pending exposes the UMI
+ * batch exactly as it would go to fgb_umi_assign (one entry per queued group with templates) and flush_with_ids
+ * completes the flush from ids / kinds / group_mi_count computed elsewhere.  The pointers of pending stay valid until
+ * the next add / flush / destroy. */
+typedef struct fgb_grouper fgb_grouper;
+fgb_status fgb_grouper_create(int device, const fgb_group_options* opt, fgb_grouper** out);
+void fgb_grouper_destroy(fgb_grouper* g);
+size_t fgb_grouper_last_error(const fgb_grouper* g, char* buf, size_t buf_len);
+fgb_status fgb_grouper_add_groups(fgb_grouper* g, const uint8_t* records, const uint64_t* rec_off,
+                                  const uint64_t* group_rec, uint64_t n_groups);
+fgb_status fgb_grouper_pending(fgb_grouper* g, const uint8_t** umis, const uint64_t** umi_off, uint64_t* n_umis,
+                               const uint64_t** call_off, uint64_t* n_calls, const uint64_t** group_off,
+                               uint64_t* n_groups);
+fgb_status fgb_grouper_flush(fgb_grouper* g, const uint8_t** out, uint64_t* out_len, uint64_t* n_records);
+fgb_status fgb_grouper_flush_with_ids(fgb_grouper* g, const uint64_t* ids, const uint8_t* kinds,
+                                      const uint64_t* group_mi_count, const uint8_t** out, uint64_t* out_len,
+                                      uint64_t* n_records);
+fgb_status fgb_grouper_stats(const fgb_grouper* g, uint64_t stats[FGB_GROUP_NSTATS]);
+/* Family sizes (templates per molecule) or position-group sizes (molecules per group) accumulated over every flush,
+ * ascending: *n entries, written only when cap >= *n (call with cap 0 to size). */
+fgb_status fgb_grouper_histogram(const fgb_grouper* g, int which, uint64_t* sizes, uint64_t* counts, uint64_t cap,
+                                 uint64_t* n);
+/* Where the last fgb_grouper_flush spent its time, in ms: [0..3] fgb_umi_last_timing of its assignment, [4] the
+ * sort, tags and output stream on the host. */
+fgb_status fgb_grouper_last_timing(const fgb_grouper* g, double ms[5]);
+
 /* sizeof() of the ABI structs as this library was compiled, so a binding can check its own layout:
  * 0 fgb_caller_options, 1 fgb_filter_params, 2 fgb_submit_options, 3 fgb_raw_columns,
  * 4 fgb_raw_read, 5 fgb_batch, 6 fgb_codec_params, 7 fgb_params, 8 fgb_duplex_filter_params,
- * 9 fgb_record_columns; 0 for an unknown id. */
+ * 9 fgb_record_columns, 10 fgb_umi_options, 11 fgb_group_options; 0 for an unknown id. */
 uint32_t fgb_struct_size(uint32_t id);
 
 #ifdef __cplusplus
