@@ -202,12 +202,13 @@ UNIT_READS = "consensus_reads/s"
 class _Caller:
     """fgb_caller_* through ctypes without copying the output (the timed call is the C-ABI itself)."""
 
-    def __init__(self, lib, device: int, n_threads: int, overlap: bool = False, zero_copy: bool = True):
+    def __init__(self, lib, device: int, n_threads: int, overlap: bool = False, zero_copy: bool = True,
+                 min_reads: int = 1):
         o = _l.FgbCallerOptions()
         o.mode = 0; o.error_rate_pre_umi = 45; o.error_rate_post_umi = 40; o.min_input_base_quality = 10
         o.min_consensus_base_quality = 2; o.produce_per_base_tags = 1; o.trim = 0
         o.consensus_call_overlapping_bases = int(overlap)
-        o.min_reads = 1; o.tag = b"MI"; o.read_name_prefix = b"fgumi"; o.read_group_id = b"A"
+        o.min_reads = min_reads; o.tag = b"MI"; o.read_name_prefix = b"fgumi"; o.read_group_id = b"A"
         o.n_threads = n_threads
         o.zero_copy_records = int(zero_copy)     # the legs pass page-locked records that stay put until the flush returns
         self._keep = o

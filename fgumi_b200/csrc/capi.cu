@@ -907,6 +907,12 @@ fgb_status submit_impl(fgb_handle* h, const fgb_batch* in, const fgb_columns* ou
         lo = std::min(lo, rr.src_off);
         hi = std::max(hi, e);
       }
+      for (uint64_t k = 0; k < n_oruns; ++k) {   // runs may touch records that yield no row: those stay resident too
+        const fgb_overlap_run& o = opt->overlap_runs[k];
+        lo = std::min(lo, std::min(o.seq1_off, o.seq2_off));
+        hi = std::max(hi, std::max(o.seq1_off + ((static_cast<uint64_t>(o.l_seq1) + 1u) >> 1) + o.l_seq1,
+                                   o.seq2_off + ((static_cast<uint64_t>(o.l_seq2) + 1u) >> 1) + o.l_seq2));
+      }
       if (hi > rec->n_bytes || lo > hi) {
         h->last_error = "fgb_record_columns: a sequence / quality span runs past the record blob";
         return FGB_ERR_LAYOUT;

@@ -787,7 +787,20 @@ fgb_status flush_simplex_direct(fgb_caller* c) {
   PhaseTrace trace;
   DLayout L;
   const fgb_status lst = lay_out_direct(c, &L);
-  if (lst != FGB_OK || !L.U) return lst;
+  if (lst != FGB_OK) return lst;
+  if (!L.U) {
+    // Nothing to vote, so nothing goes to the device.  The queued overlap runs (pairs the group rules rejected)
+    // still count, as the reference co-calls every pair (simplex.rs:395-398); their rewritten bases would feed no
+    // row, so the counters come from a read-only pass over the staged records (or the caller's own blob).
+    const uint8_t* const stage0 = c->zc_base ? c->zc_base : static_cast<const uint8_t*>(c->stage.p);
+    for (const DSeg& sg : c->segs)
+      for (uint64_t k = sg.o0; k < sg.o1; ++k) {
+        const fgb_overlap_run& r = sg.ctx->dplan.oruns[k];
+        const uint8_t* s1 = stage0 + r.seq1_off; const uint8_t* s2 = stage0 + r.seq2_off;
+        c->overlap.count_run(s1, s1 + (r.l_seq1 + 1ull) / 2, r.o1, s2, s2 + (r.l_seq2 + 1ull) / 2, r.o2, r.len);
+      }
+    return FGB_OK;
+  }
   const size_t NS = c->segs.size();
   const std::vector<uint64_t> &ub = L.ub, &bb = L.bb;
   const uint64_t U = L.U, R = L.R, n_bytes = L.n_bytes, no = L.n_out;

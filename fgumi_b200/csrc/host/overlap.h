@@ -161,6 +161,15 @@ class Caller {
   Agreement agreement() const { return agree_; }
   Disagreement disagreement() const { return disagree_; }
 
+  // The counters one run adds, without writing a base: for runs whose pairs yield no row, so nothing is built from
+  // the rewritten bases (the counters still follow the reference, which co-calls every pair of every group).
+  void count_run(const uint8_t* seq1, const uint8_t* q1, int64_t o1, const uint8_t* seq2, const uint8_t* q2, int64_t o2,
+                 int64_t len) {
+    // run<false> only reads through the pointers
+    run<false>(const_cast<uint8_t*>(seq1), const_cast<uint8_t*>(q1), o1, const_cast<uint8_t*>(seq2),
+               const_cast<uint8_t*>(q2), o2, len);
+  }
+
   // apply_overlapping_consensus: pair primary R1/R2 records of one group by name; the last record
   // seen for a (name, segment) wins, as in the reference's map insertion.
   void apply_group(uint8_t* records, const uint64_t* off, uint32_t n) {
@@ -207,6 +216,7 @@ class Caller {
     return true;
   }
 
+  template <bool kWrite = true>
   void run(uint8_t* seq1, uint8_t* q1, int64_t o1, uint8_t* seq2, uint8_t* q2, int64_t o2, int64_t len) {
     for (int64_t k = 0; k < len; ++k, ++o1, ++o2) {
       const uint8_t c1 = get_code(seq1, o1), c2 = get_code(seq2, o2);
@@ -219,7 +229,7 @@ class Caller {
         const uint8_t nq = agree_ == kAgreeConsensus
                                ? static_cast<uint8_t>(std::min<unsigned>(unsigned(x) + unsigned(y), 93u))
                                : std::max(x, y);
-        q1[o1] = nq; q2[o2] = nq;
+        if constexpr (kWrite) { q1[o1] = nq; q2[o2] = nq; }
         if (nq != x || nq != y) ++stats.bases_corrected;
         continue;
       }
@@ -228,18 +238,16 @@ class Caller {
         uint8_t code = 15, q = 2;
         if (x > y) { code = c1; q = std::max<uint8_t>(static_cast<uint8_t>(x - y), 2); }
         else if (y > x) { code = c2; q = std::max<uint8_t>(static_cast<uint8_t>(y - x), 2); }
-        set_code(seq1, o1, code); set_code(seq2, o2, code);
-        q1[o1] = q; q2[o2] = q;
+        if constexpr (kWrite) { set_code(seq1, o1, code); set_code(seq2, o2, code); q1[o1] = q; q2[o2] = q; }
         stats.bases_corrected += 2;
       } else if (disagree_ == kDisagreeMaskBoth || x == y) {
-        set_code(seq1, o1, 15); set_code(seq2, o2, 15);
-        q1[o1] = 2; q2[o2] = 2;
+        if constexpr (kWrite) { set_code(seq1, o1, 15); set_code(seq2, o2, 15); q1[o1] = 2; q2[o2] = 2; }
         stats.bases_corrected += 2;
       } else if (x < y) {
-        set_code(seq1, o1, 15); q1[o1] = 2;
+        if constexpr (kWrite) { set_code(seq1, o1, 15); q1[o1] = 2; }
         ++stats.bases_corrected;
       } else {
-        set_code(seq2, o2, 15); q2[o2] = 2;
+        if constexpr (kWrite) { set_code(seq2, o2, 15); q2[o2] = 2; }
         ++stats.bases_corrected;
       }
     }

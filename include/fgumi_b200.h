@@ -289,7 +289,10 @@ enum { FGB_OVERLAP_DISAGREE_CONSENSUS = 0, FGB_OVERLAP_DISAGREE_MASK_BOTH = 1,
  * the headers and CIGARs, the device applies the per-base rule): `len` bases of the record whose packed sequence
  * starts at seq1_off (l_seq1 bases, qualities behind them) from read offset o1, against the record at seq2_off
  * from o2.  The runs of one pair are consecutive; all but the first carry FGB_RUN_CONTINUES (one thread walks a
- * pair, so two runs never write the same packed byte at once). */
+ * pair, so two runs never write the same packed byte at once).  A run may touch records that yield no row (a pair
+ * whose reads the group rules rejected: the reference co-calls every pair and counts it): the call keeps every
+ * run's sequence and quality fields resident next to the reads' and applies and counts every run.  A batch with no
+ * tiles enqueues nothing, so its runs are neither applied nor counted; count those on the host. */
 typedef struct fgb_overlap_run {
   uint64_t seq1_off, seq2_off;
   uint32_t l_seq1, l_seq2;

@@ -1,6 +1,7 @@
 // Test harness (not product code): the product's record-level callers end to end on the CPU -- host prep,
 // flush, record assembly, filter -- with tests/native/mock_engine.cpp standing in for the GPU engine.
 // usage: caller_e2e <groups file> <threads> <variant> <output file>
+// variant 0: plain, 1: with the filter stage, 2: simplex with min_reads = 2.  Prints the count and every statistic.
 // Built and driven by tests/test_caller_planning.py::test_callers_end_to_end_on_a_mock_engine.
 #include <cstdio>
 #include <cstdlib>
@@ -40,6 +41,7 @@ int main(int argc, char** argv) {
   o.zero_copy_records = 1;                       // used when the mock engine reports page-locked memory (FGB_MOCK_PINNED)
   o.codec.single_strand_qual = -1; o.codec.outer_bases_qual = -1; o.codec.outer_bases_length = 5;
   o.codec.max_duplex_disagreements = 0xFFFFFFFFu; o.codec.max_duplex_disagreement_rate = 1.0;
+  if (variant == 2) o.min_reads = 2;             // simplex, every group one pair: a batch the group rules reject whole
   if (variant == 1 && mode == 0) {
     o.filter_enabled = 1;
     o.filter.min_reads = 1; o.filter.max_read_error_rate = 0.2; o.filter.max_base_error_rate = 0.3;

@@ -475,3 +475,24 @@ def test_callers_end_to_end_on_a_mock_engine(tmp_path, sanitizer):
                                    env=dict(env, FGB_MOCK_PINNED="1"))
                 assert r.returncode == 0 and r.stdout.startswith("ok count"), (r.stdout[-300:], r.stderr[-3000:])
                 assert open(outp, "rb").read() == want
+    # a batch the group rules reject whole (min_reads = 2, every group one overlapping pair): nothing is voted, yet
+    # the pre-pass counters must match the reference, which co-calls every pair of every group; two flushes
+    from tests.test_overlap_device import group, oracle_run, stat_view
+    groups = [group(rng, "single", g, 2) for g in range(40)]
+    path = tmp_path / "groups_rejected.bin"
+    with open(path, "wb") as f:
+        f.write(struct.pack("<II", 0, len(groups)))
+        for g in groups:
+            f.write(struct.pack("<I", len(g)))
+            for rec in g:
+                f.write(struct.pack("<I", len(rec)) + bytes(rec))
+    want, count, s, ov = oracle_run(groups, 2)
+    assert count == 0 and ov[0] > 1000
+    for threads, extra in ((1, {}), (4, {}), (4, {"FGB_MOCK_PINNED": "1"})):
+        outp = tmp_path / "out_rejected.bin"
+        r = subprocess.run([str(exe), str(path), str(threads), "2", str(outp)], capture_output=True, text=True,
+                           timeout=900, env=dict(env, **extra))
+        assert r.returncode == 0 and r.stdout.startswith("ok count 0 "), (threads, extra, r.stdout[-300:], r.stderr[-3000:])
+        assert open(outp, "rb").read() == b""
+        st = dict(zip(fg.lib.STAT_NAMES, (int(x) for x in r.stdout.split()[3:])))
+        assert {k: st[k] for k in stat_view(s, ov)} == stat_view(s, ov, 2), (threads, extra)
