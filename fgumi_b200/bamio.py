@@ -148,6 +148,47 @@ def group_header(input_text: bytes, command_line: str = "fgumi_b200 group") -> b
     return ("\n".join([ln for ln in lines if ln] + [pg]) + "\n").encode()
 
 
+def sort_header(input_text: bytes, order: str, command_line: str = "fgumi_b200 sort") -> bytes:
+    """`fgumi sort`'s output header (sort/mod.rs:72-129, raw.rs:1530-1535): the input header with one @PG chained as
+    group_header chains it, then SO / GO / SS of the @HD line removed and set again -- SO:coordinate, or SO:unsorted
+    GO:query SS:template-coordinate -- keeping VN and the other @HD fields; an @HD line is created when there is none."""
+    tags = {"coordinate": [("SO", "coordinate")],
+            "template-coordinate": [("SO", "unsorted"), ("GO", "query"), ("SS", "template-coordinate")]}[order]
+    lines = group_header(input_text, command_line).decode("utf-8", "replace").rstrip("\n").split("\n")
+    at = next((i for i, ln in enumerate(lines) if ln.startswith("@HD")), None)
+    fields = [] if at is None else [f for f in lines[at].split("\t")[1:] if f[:3] not in ("SO:", "GO:", "SS:")]
+    hd = "\t".join(["@HD"] + fields + ["%s:%s" % kv for kv in tags])
+    if at is None:
+        lines.insert(0, hd)
+    else:
+        lines[at] = hd
+    return ("\n".join(lines) + "\n").encode()
+
+
+def sort_file(in_path: str, out_path: str, sorter, n_threads: int = 4, level: int = 1) -> Dict[str, float]:
+    """`fgumi sort -i in.bam -o out.bam --order <sorter's order>` with an existing sort.RecordSorter.  Returns the
+    phase timings: read / inflate / split (read_bam), device (the sort call, with the sorter's own phases), compress."""
+    lib = _l.load()
+    text, bodies, rec_off, tm = read_bam(in_path, n_threads)
+    t0 = time.perf_counter()
+    stream = sorter.sort(text, bodies, rec_off)
+    t1 = time.perf_counter()
+    payload = mapped_bam_header(sort_header(text, sorter.order)) + stream
+    cap = lib.fgb_bgzf_bound(len(payload))
+    comp = np.empty(cap, dtype=np.uint8)
+    cn = C.c_size_t()
+    t2 = time.perf_counter()
+    st = lib.fgb_bgzf_compress(payload, len(payload), level, n_threads, 1, comp.ctypes.data, cap, C.addressof(cn))
+    if st != 0:
+        raise _l.FgbError(st, "fgb_bgzf_compress")
+    t3 = time.perf_counter()
+    comp[:cn.value].tofile(out_path)
+    tm.update({"device_s": t1 - t0, "compress_s": t3 - t2, "input_records": float(len(rec_off) - 1),
+               "output_bytes": float(len(payload))})
+    tm.update({k: v for k, v in sorter.last_timing().items()})
+    return tm
+
+
 def check_group_sort_order(text: bytes, allow_unmapped: bool) -> None:
     """group.rs:797-817: template-coordinate input (SO:unsorted GO:query, SS ending in template-coordinate if
     present), or queryname-sorted input with --allow-unmapped."""

@@ -21,8 +21,10 @@
 #include "inflate_kernel.cuh"
 #include "host_tables.h"
 #include "planner.h"
+#include "sort_kernels.cuh"
 #include "umi_kernels.cuh"
 #include "unpack_kernels.cuh"
+#include "host/sort_device.h"
 #include "host/umi_host.h"
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -123,6 +125,7 @@ struct fgb_handle {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;   // around the count and fill passes
     double timing[4] = {0, 0, 0, 0};                 // fgb_umi_last_timing
   } umi;
+  double sort_timing[6] = {0, 0, 0, 0, 0, 0};        // fgb_sort_last_timing
 };
 
 namespace {
@@ -1693,3 +1696,67 @@ fgb_status fgb_umi_edges(fgb_handle* h, const fgb_umi_options* opt, const uint8_
 }
 
 }  // extern "C"
+
+// ---- record sort (sort_kernels.cuh; the driver is host/sort_host.cpp) --------------------------------------------
+namespace fgb {
+namespace sortdev {
+
+HandleInfo info(fgb_handle* h) {
+  return HandleInfo{h->device, h->sm_count, h->slots[0].stream, h->submit_pending, &h->last_error, h->sort_timing};
+}
+
+namespace {
+unsigned blocks(uint32_t n) { return (n + kSortThreads - 1) / kSortThreads; }
+}  // namespace
+
+cudaError_t keys(const uint8_t* rec, const uint64_t* off, uint64_t base, uint32_t n, const sortk::Ctx& ctx, int words,
+                 uint64_t* keys, uint32_t* size, unsigned long long* and_or, cudaStream_t s) {
+  if (!n) return cudaSuccess;
+  if (words == 1) sort_key_kernel<1><<<blocks(n), kSortThreads, 0, s>>>(rec, off, base, n, ctx, keys, size, and_or);
+  else sort_key_kernel<sortk::kWords><<<blocks(n), kSortThreads, 0, s>>>(rec, off, base, n, ctx, keys, size, and_or);
+  return cudaGetLastError();
+}
+
+cudaError_t word_gather(const uint64_t* word, const uint32_t* perm, uint32_t n, uint64_t* dst, cudaStream_t s) {
+  if (!n) return cudaSuccess;
+  sort_word_gather_kernel<<<blocks(n), kSortThreads, 0, s>>>(word, perm, n, dst, nullptr);
+  return cudaGetLastError();
+}
+
+cudaError_t iota(uint32_t* v, uint32_t n, cudaStream_t s) {
+  if (!n) return cudaSuccess;
+  sort_word_gather_kernel<<<blocks(n), kSortThreads, 0, s>>>(nullptr, nullptr, n, nullptr, v);
+  return cudaGetLastError();
+}
+
+cudaError_t key_rows(const uint64_t* keys, const uint32_t* perm, uint32_t n, int words, uint64_t* rows, cudaStream_t s) {
+  if (!n) return cudaSuccess;
+  sort_key_rows_kernel<<<blocks(n), kSortThreads, 0, s>>>(keys, perm, n, words, rows);
+  return cudaGetLastError();
+}
+
+cudaError_t radix_pass(void* temp, size_t* temp_bytes, const uint64_t* kin, uint64_t* kout, const uint32_t* vin,
+                       uint32_t* vout, uint32_t n, int begin, int end, cudaStream_t s) {
+  return cub::DeviceRadixSort::SortPairs(temp, *temp_bytes, kin, kout, vin, vout, static_cast<int>(n), begin, end, s);
+}
+
+cudaError_t out_offsets(void* temp, size_t* temp_bytes, const uint32_t* size, const uint32_t* perm, uint32_t n,
+                        uint64_t* out_size, uint64_t* out_off, cudaStream_t s) {
+  if (!temp) return cub::DeviceScan::ExclusiveSum(nullptr, *temp_bytes, out_size, out_off, static_cast<int>(n) + 1, s);
+  if (n) sort_out_size_kernel<<<blocks(n), kSortThreads, 0, s>>>(size, perm, n, out_size);
+  cudaError_t e = cudaMemsetAsync(out_size + n, 0, sizeof(uint64_t), s);
+  if (e != cudaSuccess) return e;
+  return cub::DeviceScan::ExclusiveSum(temp, *temp_bytes, out_size, out_off, static_cast<int>(n) + 1, s);
+}
+
+cudaError_t gather(const uint8_t* rec, const uint64_t* off, uint64_t base, const uint32_t* perm,
+                   const uint64_t* out_off, uint32_t n, uint8_t* out, int sm_count, cudaStream_t s) {
+  if (!n) return cudaSuccess;
+  const uint64_t want = (static_cast<uint64_t>(n) * 32 + kSortThreads - 1) / kSortThreads;   // one warp per record
+  const unsigned grid = static_cast<unsigned>(std::min<uint64_t>(want, static_cast<uint64_t>(sm_count) * 16));
+  sort_gather_kernel<<<grid, kSortThreads, 0, s>>>(rec, off, base, perm, out_off, n, out);
+  return cudaGetLastError();
+}
+
+}  // namespace sortdev
+}  // namespace fgb

@@ -13,6 +13,7 @@
 #include <cstdint>
 #include <cstring>
 #include <string>
+#include <string_view>
 #include <utility>
 #include <vector>
 
@@ -165,6 +166,33 @@ inline void find_string_tags(const View& v, const char (*want)[2], int n_want, c
     }
     if (hit >= 0) { seen |= 1u << hit; --left; }
     p += 3 + size;
+  }
+}
+
+// The @RG lines of a SAM header text: fn(id, lb, has_lb) for each line with an ID, in header order (the last ID: / LB:
+// field of a line wins).  Each caller numbers the libraries its own way.
+template <class F>
+inline void for_each_read_group(std::string_view text, F&& fn) {
+  size_t p = 0;
+  while (p < text.size()) {
+    size_t e = text.find('\n', p);
+    if (e == std::string_view::npos) e = text.size();
+    std::string_view line = text.substr(p, e - p);
+    if (!line.empty() && line.back() == '\r') line.remove_suffix(1);
+    p = e + 1;
+    if (line.substr(0, 4) != "@RG\t") continue;
+    std::string_view id, lb;
+    bool has_id = false, has_lb = false;
+    size_t q = 4;
+    while (q <= line.size()) {
+      size_t t = line.find('\t', q);
+      if (t == std::string_view::npos) t = line.size();
+      std::string_view f = line.substr(q, t - q);
+      if (f.substr(0, 3) == "ID:") { id = f.substr(3); has_id = true; }
+      else if (f.substr(0, 3) == "LB:") { lb = f.substr(3); has_lb = true; }
+      q = t + 1;
+    }
+    if (has_id) fn(id, lb, has_lb);
   }
 }
 

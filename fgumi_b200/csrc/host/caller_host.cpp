@@ -2711,6 +2711,7 @@ uint32_t fgb_struct_size(uint32_t id) {
     case 9: return sizeof(fgb_record_columns);
     case 10: return sizeof(fgb_umi_options);
     case 11: return sizeof(fgb_group_options);
+    case 12: return sizeof(fgb_sort_options);
     default: return 0;
   }
 }

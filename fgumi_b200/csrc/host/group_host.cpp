@@ -99,30 +99,12 @@ struct PosKey {
 // @RG lines, an RG without LB is library "unknown" = 0, as is an RG the header does not declare.
 std::map<std::string, uint16_t> library_index(std::string_view text) {
   std::map<std::string, uint16_t> lib_of_name{{"unknown", 0}}, lib_of_rg;
-  size_t p = 0;
-  while (p < text.size()) {
-    size_t e = text.find('\n', p);
-    if (e == std::string_view::npos) e = text.size();
-    std::string_view line = text.substr(p, e - p);
-    if (!line.empty() && line.back() == '\r') line.remove_suffix(1);
-    p = e + 1;
-    if (line.substr(0, 4) != "@RG\t") continue;
-    std::string id, lb = "unknown";
-    bool has_id = false;
-    size_t q = 4;
-    while (q <= line.size()) {
-      size_t t = line.find('\t', q);
-      if (t == std::string_view::npos) t = line.size();
-      std::string_view f = line.substr(q, t - q);
-      if (f.substr(0, 3) == "ID:") { id = std::string(f.substr(3)); has_id = true; }
-      else if (f.substr(0, 3) == "LB:") lb = std::string(f.substr(3));
-      q = t + 1;
-    }
-    if (!has_id) continue;
-    auto it = lib_of_name.find(lb);
-    if (it == lib_of_name.end()) it = lib_of_name.emplace(lb, static_cast<uint16_t>(lib_of_name.size())).first;
-    lib_of_rg[id] = it->second;
-  }
+  bam::for_each_read_group(text, [&](std::string_view id, std::string_view lb, bool has_lb) {
+    const std::string name = has_lb ? std::string(lb) : "unknown";
+    auto it = lib_of_name.find(name);
+    if (it == lib_of_name.end()) it = lib_of_name.emplace(name, static_cast<uint16_t>(lib_of_name.size())).first;
+    lib_of_rg[std::string(id)] = it->second;
+  });
   return lib_of_rg;
 }
 

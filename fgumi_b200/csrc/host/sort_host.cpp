@@ -1,0 +1,429 @@
+// `fgumi sort` (coordinate and template-coordinate) from raw BAM records: the header's library table, the host key
+// and verify entry points, and the driver of the device sort (fgb_sort_records): runs that fit a device budget, each
+// uploaded through page-locked staging, keyed, sorted by stable radix passes over the key words that vary and gathered
+// into a [u32 block_size][record] stream on the device; several runs are merged on the host.  The key functions are
+// ../sort_keys.h; the kernels and CUB calls sit behind sort_device.h in capi.cu.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <chrono>
+#include <cstring>
+#include <map>
+#include <new>
+#include <string>
+#include <string_view>
+#include <vector>
+
+#include "../../../include/fgumi_b200.h"
+#include "../sort_keys.h"
+#include "bam.h"
+#include "sort_device.h"
+#include "umi_host.h"
+
+namespace {
+
+namespace sk = fgb::sortk;
+namespace dev = fgb::sortdev;
+
+static_assert(FGB_SORT_COORDINATE == sk::kCoordinate && FGB_SORT_TEMPLATE_COORDINATE == sk::kTemplateCoordinate,
+              "sort orders");
+constexpr uint64_t kNone = UINT64_MAX;
+constexpr uint64_t kStageBytes = 64ull << 20;   // one page-locked staging buffer (two alternate)
+
+// LibraryLookup::from_header (raw.rs:237-283): the distinct LB values sorted bytewise and numbered from 1; each RG ID
+// maps to its LB's ordinal, an RG without LB to that of "" (0 unless some LB is empty).  IDs are kept sorted bytewise
+// (std::string compares as unsigned bytes) so that the key functions look them up by binary search.
+struct Lookup {
+  std::vector<uint8_t> bytes;
+  std::vector<uint32_t> off{0};
+  std::vector<uint32_t> lib;
+};
+
+Lookup library_lookup(std::string_view text) {
+  std::map<std::string, std::string> lb_of_rg;   // an RG without LB maps to ""
+  std::vector<std::string> libs;
+  fgb::bam::for_each_read_group(text, [&](std::string_view id, std::string_view lb, bool has_lb) {
+    lb_of_rg[std::string(id)] = std::string(lb);
+    if (has_lb) libs.emplace_back(lb);
+  });
+  std::sort(libs.begin(), libs.end());
+  libs.erase(std::unique(libs.begin(), libs.end()), libs.end());
+  Lookup l;
+  for (const auto& [id, lb] : lb_of_rg) {
+    l.bytes.insert(l.bytes.end(), id.begin(), id.end());
+    l.off.push_back(static_cast<uint32_t>(l.bytes.size()));
+    const auto it = std::lower_bound(libs.begin(), libs.end(), lb);
+    l.lib.push_back(it != libs.end() && *it == lb ? static_cast<uint32_t>(it - libs.begin()) + 1 : 0);
+  }
+  return l;
+}
+
+bool options_ok(const fgb_sort_options* o) {
+  if (!o || o->order > FGB_SORT_TEMPLATE_COORDINATE) return false;
+  return (o->cell_tag[0] == 0) == (o->cell_tag[1] == 0);
+}
+
+sk::Ctx make_ctx(const fgb_sort_options& o, const uint8_t* bytes, const uint32_t* off, const uint32_t* lib, uint32_t n_rg) {
+  sk::Ctx c{};
+  c.rg_bytes = bytes; c.rg_off = off; c.rg_lib = lib; c.n_rg = n_rg;
+  c.order = o.order;
+  c.has_cell = o.order == FGB_SORT_TEMPLATE_COORDINATE && o.cell_tag[0] != 0;
+  c.cell[0] = static_cast<uint8_t>(o.cell_tag[0]);
+  c.cell[1] = static_cast<uint8_t>(o.cell_tag[1]);
+  return c;
+}
+
+int key_words(const fgb_sort_options& o) { return o.order == FGB_SORT_COORDINATE ? 1 : sk::kWords; }
+
+// Each record holds its 32-byte fixed part and rec_off ascends; else *bad = the first offending record.
+bool records_ok(const uint64_t* rec_off, uint64_t n, uint64_t* bad) {
+  for (uint64_t i = 0; i < n; ++i)
+    if (rec_off[i + 1] < rec_off[i] || rec_off[i + 1] - rec_off[i] < 32) { if (bad) *bad = i; return false; }
+  return true;
+}
+
+bool args_ok(const fgb_sort_options* opt, const char* header_text, size_t header_len, const uint8_t* records,
+             const uint64_t* rec_off, uint64_t n) {
+  return options_ok(opt) && (!header_len || header_text) && rec_off && (!n || records);
+}
+
+// Keys of every record, row-major (5 words per record), on n_threads host threads.
+void host_keys(const fgb_sort_options& o, std::string_view header, const uint8_t* records, const uint64_t* rec_off,
+               uint64_t n, uint64_t* keys) {
+  const Lookup l = library_lookup(header);
+  const sk::Ctx c = make_ctx(o, l.bytes.data(), l.off.data(), l.lib.data(), static_cast<uint32_t>(l.lib.size()));
+  const uint64_t t = std::max<uint32_t>(o.n_threads, 1);
+  fgb_umi::parallel_for(t, o.n_threads, [&](uint64_t w) {
+    for (uint64_t i = n * w / t, e = n * (w + 1) / t; i < e; ++i)
+      sk::record_key(records + rec_off[i], rec_off[i + 1] - rec_off[i], c, keys + sk::kWords * i);
+  });
+}
+
+// memcpy on n_threads host threads (the staging copies are what bounds the upload and download)
+void par_copy(uint8_t* dst, const uint8_t* src, uint64_t n, uint32_t n_threads) {
+  const uint64_t t = std::min<uint64_t>(std::max<uint32_t>(n_threads, 1), std::max<uint64_t>(n >> 22, 1));
+  fgb_umi::parallel_for(t, n_threads, [&](uint64_t w) {
+    const uint64_t b = n * w / t, e = n * (w + 1) / t;
+    if (e > b) std::memcpy(dst + b, src + b, e - b);
+  });
+}
+
+// Everything one fgb_sort_records call allocates, freed on every way out.
+struct Resources {
+  std::vector<void*> dev;
+  uint8_t* stage[2] = {nullptr, nullptr};
+  cudaEvent_t staged[2] = {nullptr, nullptr};
+  cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+  ~Resources() {
+    for (void* p : dev) cudaFree(p);
+    for (auto* s : stage) if (s) cudaFreeHost(s);
+    for (auto e : staged) if (e) cudaEventDestroy(e);
+    for (auto e : ev) if (e) cudaEventDestroy(e);
+  }
+  template <class T>
+  cudaError_t alloc(T** p, uint64_t count) {
+    void* q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, std::max<uint64_t>(count, 1) * sizeof(T));
+    if (e == cudaSuccess) dev.push_back(q);
+    *p = static_cast<T*>(q);
+    return e;
+  }
+};
+
+struct Driver {
+  dev::HandleInfo hi;
+  const fgb_sort_options& o;
+  uint32_t threads;
+  Resources r;
+  cudaStream_t s;
+
+  fgb_status fail(cudaError_t e, const char* what) {
+    cudaGetLastError();   // a failed allocation must not surface in the handle's next launch check
+    *hi.last_error = std::string("fgb_sort_records: ") + what + ": " + cudaGetErrorString(e);
+    return e == cudaErrorMemoryAllocation ? FGB_ERR_NOMEM : FGB_ERR_CUDA;
+  }
+
+  // host -> device through the two staging buffers: the copy into one overlaps the transfer out of the other
+  cudaError_t upload(uint8_t* dst, const uint8_t* src, uint64_t n) {
+    for (uint64_t at = 0, k = 0; at < n; at += kStageBytes, ++k) {
+      const int b = static_cast<int>(k & 1);
+      const uint64_t len = std::min(kStageBytes, n - at);
+      cudaError_t e = cudaEventSynchronize(r.staged[b]);
+      if (e != cudaSuccess) return e;
+      par_copy(r.stage[b], src + at, len, threads);
+      if ((e = cudaMemcpyAsync(dst + at, r.stage[b], len, cudaMemcpyHostToDevice, s)) != cudaSuccess) return e;
+      if ((e = cudaEventRecord(r.staged[b], s)) != cudaSuccess) return e;
+    }
+    return cudaStreamSynchronize(s);
+  }
+
+  // device -> host the same way: the transfer into one buffer overlaps the copy out of the other
+  cudaError_t download(uint8_t* dst, const uint8_t* src, uint64_t n) {
+    uint64_t prev_at = 0, prev_len = 0;
+    int prev = -1;
+    for (uint64_t at = 0, k = 0; at < n; at += kStageBytes, ++k) {
+      const int b = static_cast<int>(k & 1);
+      const uint64_t len = std::min(kStageBytes, n - at);
+      cudaError_t e = cudaMemcpyAsync(r.stage[b], src + at, len, cudaMemcpyDeviceToHost, s);
+      if (e != cudaSuccess || (e = cudaEventRecord(r.staged[b], s)) != cudaSuccess) return e;
+      if (prev >= 0) {
+        if ((e = cudaEventSynchronize(r.staged[prev])) != cudaSuccess) return e;
+        par_copy(dst + prev_at, r.stage[prev], prev_len, threads);
+      }
+      prev = b; prev_at = at; prev_len = len;
+    }
+    if (prev >= 0) {
+      const cudaError_t e = cudaEventSynchronize(r.staged[prev]);
+      if (e != cudaSuccess) return e;
+      par_copy(dst + prev_at, r.stage[prev], prev_len, threads);
+    }
+    return cudaSuccess;
+  }
+};
+
+double ms_since(std::chrono::steady_clock::time_point t) {
+  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
+}
+
+fgb_status sort_impl(fgb_handle* h, const fgb_sort_options& o, std::string_view header, const uint8_t* records,
+                     const uint64_t* rec_off, uint64_t n, uint8_t* out) {
+  Driver d{dev::info(h), o, std::max<uint32_t>(o.n_threads, 1), {}, nullptr};
+  d.s = d.hi.stream;
+  double* tm = d.hi.timing;
+  const int W = key_words(o);
+  cudaError_t e = cudaSetDevice(d.hi.device);
+  if (e != cudaSuccess) return d.fail(e, "cudaSetDevice");
+  // runs: as many records as fit the budget (input and output bytes, keys, permutations and scan / sort scratch)
+  uint64_t budget = o.device_bytes;
+  if (!budget) {
+    size_t free_b = 0, total_b = 0;
+    if ((e = cudaMemGetInfo(&free_b, &total_b)) != cudaSuccess) return d.fail(e, "cudaMemGetInfo");
+    budget = free_b - free_b / 8 - std::min<uint64_t>(free_b / 8, 512ull << 20);
+  }
+  const uint64_t per_record = 68 + 8ull * W;
+  std::vector<uint64_t> run_begin{0};
+  uint64_t max_n = 0, max_bytes = 0;
+  for (uint64_t b = 0; b < n;) {
+    uint64_t i = b + 1;   // at least one record per run
+    while (i < n && i - b < INT32_MAX &&
+           2 * (rec_off[i + 1] - rec_off[b]) + (i + 1 - b) * (per_record + 4) <= budget) ++i;
+    max_n = std::max(max_n, i - b);
+    max_bytes = std::max(max_bytes, rec_off[i] - rec_off[b]);
+    run_begin.push_back(i);
+    b = i;
+  }
+  const uint64_t n_runs = run_begin.size() - 1;
+  // buffers for the largest run
+  const Lookup l = library_lookup(header);
+  uint8_t *d_rec, *d_out, *d_rg, *d_temp;
+  uint64_t *d_off, *d_keys, *d_rows = nullptr, *d_ktmp[2], *d_osize, *d_ooff;
+  uint32_t *d_size, *d_perm[2], *d_rgoff, *d_rglib;
+  unsigned long long* d_andor;
+  const uint32_t mn = static_cast<uint32_t>(max_n);
+  size_t t_sort = 0, t_scan = 0;
+  if ((e = dev::radix_pass(nullptr, &t_sort, nullptr, nullptr, nullptr, nullptr, mn, 0, 64, d.s)) != cudaSuccess ||
+      (e = dev::out_offsets(nullptr, &t_scan, nullptr, nullptr, mn, nullptr, nullptr, d.s)) != cudaSuccess)
+    return d.fail(e, "CUB temp storage");
+  if ((e = d.r.alloc(&d_rec, max_bytes + 16)) != cudaSuccess || (e = d.r.alloc(&d_out, max_bytes + 4 * max_n)) ||
+      (e = d.r.alloc(&d_off, max_n + 1)) || (e = d.r.alloc(&d_keys, W * max_n)) ||
+      (e = d.r.alloc(&d_ktmp[0], max_n)) || (e = d.r.alloc(&d_ktmp[1], max_n)) ||
+      (e = d.r.alloc(&d_osize, max_n + 1)) || (e = d.r.alloc(&d_ooff, max_n + 1)) || (e = d.r.alloc(&d_size, max_n)) ||
+      (e = d.r.alloc(&d_perm[0], max_n)) || (e = d.r.alloc(&d_perm[1], max_n)) ||
+      (e = d.r.alloc(&d_rg, l.bytes.size())) || (e = d.r.alloc(&d_rgoff, l.off.size())) ||
+      (e = d.r.alloc(&d_rglib, l.lib.size())) || (e = d.r.alloc(&d_andor, 2 * W)) ||
+      (e = d.r.alloc(&d_temp, std::max(t_sort, t_scan) + 16)) || (n_runs > 1 && (e = d.r.alloc(&d_rows, W * max_n))))
+    return d.fail(e, "cudaMalloc");
+  const uint64_t stage = std::min<uint64_t>(kStageBytes, std::max(max_bytes + 4 * max_n, (max_n + 1) * 8));
+  for (int b = 0; b < 2; ++b) {
+    if ((e = cudaHostAlloc(reinterpret_cast<void**>(&d.r.stage[b]), stage, cudaHostAllocDefault)) != cudaSuccess)
+      return d.fail(e, "cudaHostAlloc");
+    if ((e = cudaEventCreateWithFlags(&d.r.staged[b], cudaEventDisableTiming)) != cudaSuccess)
+      return d.fail(e, "cudaEventCreate");
+  }
+  for (auto& ev : d.r.ev)
+    if ((e = cudaEventCreate(&ev)) != cudaSuccess) return d.fail(e, "cudaEventCreate");
+  if ((!l.bytes.empty() && (e = cudaMemcpy(d_rg, l.bytes.data(), l.bytes.size(), cudaMemcpyHostToDevice))) ||
+      (e = cudaMemcpy(d_rgoff, l.off.data(), l.off.size() * 4, cudaMemcpyHostToDevice)) ||
+      (!l.lib.empty() && (e = cudaMemcpy(d_rglib, l.lib.data(), l.lib.size() * 4, cudaMemcpyHostToDevice))))
+    return d.fail(e, "cudaMemcpy");
+  const sk::Ctx ctx = make_ctx(o, d_rg, d_rgoff, d_rglib, static_cast<uint32_t>(l.lib.size()));
+  // several runs: each run's sorted stream and its keys in sorted order (row-major) come back for the merge
+  std::vector<uint8_t> run_stream;
+  std::vector<std::vector<uint64_t>> run_keys(n_runs > 1 ? n_runs : 0);
+  if (n_runs > 1) run_stream.resize(rec_off[n] - rec_off[0] + 4 * n);
+  for (uint64_t x = 0; x < n_runs; ++x) {
+    const uint64_t b = run_begin[x], nr64 = run_begin[x + 1] - b;
+    const uint32_t nr = static_cast<uint32_t>(nr64);
+    const uint64_t base = rec_off[b], bytes = rec_off[b + nr64] - base, out_at = base - rec_off[0] + 4 * b;
+    auto t0 = std::chrono::steady_clock::now();
+    if ((e = d.upload(d_rec, records + base, bytes)) != cudaSuccess ||
+        (e = d.upload(reinterpret_cast<uint8_t*>(d_off), reinterpret_cast<const uint8_t*>(rec_off + b), (nr64 + 1) * 8)))
+      return d.fail(e, "upload");
+    tm[0] += ms_since(t0);
+    unsigned long long init[2 * sk::kWords];
+    for (int w = 0; w < W; ++w) { init[2 * w] = ~0ull; init[2 * w + 1] = 0; }
+    unsigned long long and_or[2 * sk::kWords];
+    if ((e = cudaMemcpyAsync(d_andor, init, 16 * W, cudaMemcpyHostToDevice, d.s)) ||
+        (e = cudaEventRecord(d.r.ev[0], d.s)) ||
+        (e = dev::keys(d_rec, d_off, base, nr, ctx, W, d_keys, d_size, d_andor, d.s)) ||
+        (e = cudaEventRecord(d.r.ev[1], d.s)) ||
+        (e = cudaMemcpyAsync(and_or, d_andor, 16 * W, cudaMemcpyDeviceToHost, d.s)) ||
+        (e = cudaStreamSynchronize(d.s)))
+      return d.fail(e, "key kernel");
+    // LSD over the words, last first, skipping constant ones and sorting only the bits that vary
+    uint32_t* perm = d_perm[0];
+    uint32_t* spare = d_perm[1];
+    bool first = true;
+    if ((e = cudaEventRecord(d.r.ev[2], d.s)) != cudaSuccess) return d.fail(e, "cudaEventRecord");
+    for (int w = W - 1; w >= 0; --w) {
+      const uint64_t diff = and_or[2 * w] ^ and_or[2 * w + 1];
+      if (!diff) continue;
+      const int lo = __builtin_ctzll(diff), hi = 64 - __builtin_clzll(diff);
+      const uint64_t* src = d_keys + static_cast<uint64_t>(w) * nr;
+      if (first) e = dev::iota(perm, nr, d.s);
+      else { e = dev::word_gather(src, perm, nr, d_ktmp[0], d.s); src = d_ktmp[0]; }
+      size_t tb = std::max(t_sort, t_scan) + 16;
+      if (e || (e = dev::radix_pass(d_temp, &tb, src, d_ktmp[1], perm, spare, nr, lo, hi, d.s)))
+        return d.fail(e, "radix pass");
+      std::swap(perm, spare);
+      first = false;
+    }
+    if (first && (e = dev::iota(perm, nr, d.s))) return d.fail(e, "iota");
+    size_t tb = std::max(t_sort, t_scan) + 16;
+    if ((e = cudaEventRecord(d.r.ev[3], d.s)) ||
+        (e = dev::out_offsets(d_temp, &tb, d_size, perm, nr, d_osize, d_ooff, d.s)) ||
+        (e = dev::gather(d_rec, d_off, base, perm, d_ooff, nr, d_out, d.hi.sm_count, d.s)) ||
+        (n_runs > 1 && (e = dev::key_rows(d_keys, perm, nr, W, d_rows, d.s))) ||
+        (e = cudaEventRecord(d.r.ev[4], d.s)) || (e = cudaStreamSynchronize(d.s)))
+      return d.fail(e, "gather");
+    float k_ms = 0, s_ms = 0, g_ms = 0;
+    cudaEventElapsedTime(&k_ms, d.r.ev[0], d.r.ev[1]);
+    cudaEventElapsedTime(&s_ms, d.r.ev[2], d.r.ev[3]);
+    cudaEventElapsedTime(&g_ms, d.r.ev[3], d.r.ev[4]);
+    tm[1] += k_ms; tm[2] += s_ms; tm[3] += g_ms;
+    t0 = std::chrono::steady_clock::now();
+    const uint64_t out_bytes = bytes + 4 * nr64;
+    if ((e = d.download((n_runs > 1 ? run_stream.data() : out) + out_at, d_out, out_bytes)))
+      return d.fail(e, "download");
+    if (n_runs > 1) {
+      run_keys[x].resize(W * nr64);
+      if ((e = cudaMemcpy(run_keys[x].data(), d_rows, W * nr64 * 8, cudaMemcpyDeviceToHost)))
+        return d.fail(e, "download");
+    }
+    tm[4] += ms_since(t0);
+  }
+  if (n_runs <= 1) return FGB_OK;
+  // k-way merge by the key words, ties by run index: a binary heap of run heads
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<uint64_t> pos(n_runs, 0), cur(n_runs);
+  for (uint64_t x = 0; x < n_runs; ++x) cur[x] = rec_off[run_begin[x]] - rec_off[0] + 4 * run_begin[x];
+  auto after = [&](uint64_t a, uint64_t b) {   // heap order: true when run a's head goes after run b's
+    const uint64_t* ka = run_keys[a].data() + W * pos[a];
+    const uint64_t* kb = run_keys[b].data() + W * pos[b];
+    for (int w = 0; w < W; ++w)
+      if (ka[w] != kb[w]) return ka[w] > kb[w];
+    return a > b;
+  };
+  std::vector<uint64_t> heap;
+  for (uint64_t x = 0; x < n_runs; ++x) heap.push_back(x);
+  std::make_heap(heap.begin(), heap.end(), after);
+  uint8_t* o_at = out;
+  while (!heap.empty()) {
+    std::pop_heap(heap.begin(), heap.end(), after);
+    const uint64_t x = heap.back();
+    uint32_t bs;
+    std::memcpy(&bs, run_stream.data() + cur[x], 4);
+    std::memcpy(o_at, run_stream.data() + cur[x], 4ull + bs);
+    o_at += 4ull + bs;
+    cur[x] += 4ull + bs;
+    if (++pos[x] < run_begin[x + 1] - run_begin[x]) std::push_heap(heap.begin(), heap.end(), after);
+    else heap.pop_back();
+  }
+  tm[5] = ms_since(t0);
+  return FGB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+fgb_status fgb_host_sort_keys(const fgb_sort_options* opt, const char* header_text, size_t header_len,
+                              const uint8_t* records, const uint64_t* rec_off, uint64_t n_records, uint64_t* keys,
+                              uint64_t* bad_record) {
+  if (!args_ok(opt, header_text, header_len, records, rec_off, n_records) || (n_records && !keys))
+    return FGB_ERR_INVALID_ARG;
+  if (bad_record) *bad_record = kNone;
+  if (!records_ok(rec_off, n_records, bad_record)) return FGB_ERR_LAYOUT;
+  try {
+    host_keys(*opt, std::string_view(header_text ? header_text : "", header_len), records, rec_off, n_records, keys);
+  } catch (const std::exception&) {
+    return FGB_ERR_NOMEM;
+  }
+  return FGB_OK;
+}
+
+fgb_status fgb_host_sort_verify(const fgb_sort_options* opt, const char* header_text, size_t header_len,
+                                const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
+                                uint64_t* violations, uint64_t* first_violation, uint64_t* bad_record) {
+  if (!args_ok(opt, header_text, header_len, records, rec_off, n_records) || !violations || !first_violation)
+    return FGB_ERR_INVALID_ARG;
+  if (bad_record) *bad_record = kNone;
+  if (!records_ok(rec_off, n_records, bad_record)) return FGB_ERR_LAYOUT;
+  try {
+    std::vector<uint64_t> k(sk::kWords * n_records);
+    host_keys(*opt, std::string_view(header_text ? header_text : "", header_len), records, rec_off, n_records, k.data());
+    const int core = opt->order == FGB_SORT_COORDINATE ? 1 : 4;   // core_cmp leaves out name_hash_upper
+    uint64_t v = 0, first = kNone;
+    for (uint64_t i = 1; i < n_records; ++i) {
+      const uint64_t* a = k.data() + sk::kWords * i;
+      const uint64_t* p = a - sk::kWords;
+      if (std::lexicographical_compare(a, a + core, p, p + core)) {
+        ++v;
+        if (first == kNone) first = i;
+      }
+    }
+    *violations = v;
+    *first_violation = first;
+  } catch (const std::exception&) {
+    return FGB_ERR_NOMEM;
+  }
+  return FGB_OK;
+}
+
+fgb_status fgb_sort_records(fgb_handle* h, const fgb_sort_options* opt, const char* header_text, size_t header_len,
+                            const uint8_t* records, const uint64_t* rec_off, uint64_t n_records, uint8_t* out,
+                            uint64_t cap, uint64_t* out_len, uint64_t* bad_record) {
+  if (!h || !out_len || !args_ok(opt, header_text, header_len, records, rec_off, n_records)) return FGB_ERR_INVALID_ARG;
+  const dev::HandleInfo hi = dev::info(h);
+  if (bad_record) *bad_record = kNone;
+  std::fill(hi.timing, hi.timing + 6, 0.0);
+  if (!records_ok(rec_off, n_records, bad_record)) {
+    *hi.last_error = "fgb_sort_records: record " + std::to_string(*bad_record) + " is shorter than 32 bytes";
+    return FGB_ERR_LAYOUT;
+  }
+  const uint64_t need = rec_off[n_records] - rec_off[0] + 4 * n_records;
+  if (cap < need || (need && !out)) {
+    *hi.last_error = "fgb_sort_records: the output needs " + std::to_string(need) + " bytes";
+    return FGB_ERR_INVALID_ARG;
+  }
+  if (hi.busy) { *hi.last_error = "fgb_sort_records: a submit has not been waited on"; return FGB_ERR_BUSY; }
+  *out_len = need;
+  if (!n_records) return FGB_OK;
+  try {
+    return sort_impl(h, *opt, std::string_view(header_text ? header_text : "", header_len), records, rec_off,
+                     n_records, out);
+  } catch (const std::bad_alloc&) {
+    *hi.last_error = "fgb_sort_records: out of host memory";
+  } catch (const std::exception& x) {
+    *hi.last_error = std::string("fgb_sort_records: ") + x.what();
+  }
+  return FGB_ERR_NOMEM;
+}
+
+fgb_status fgb_sort_last_timing(const fgb_handle* h, double ms[6]) {
+  if (!h || !ms) return FGB_ERR_INVALID_ARG;
+  std::memcpy(ms, dev::info(const_cast<fgb_handle*>(h)).timing, 6 * sizeof(double));
+  return FGB_OK;
+}
+
+}  // extern "C"

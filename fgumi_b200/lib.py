@@ -210,6 +210,14 @@ GROUP_STAT_NAMES = ("total_records", "accepted_records", "discarded_non_pf", "di
 FGB_GROUP_HIST_FAMILY, FGB_GROUP_HIST_POSITION = 0, 1
 
 
+FGB_SORT_COORDINATE, FGB_SORT_TEMPLATE_COORDINATE = 0, 1
+
+
+class FgbSortOptions(C.Structure):
+    _fields_ = [("order", C.c_uint32), ("n_threads", C.c_uint32), ("cell_tag", C.c_char * 2),
+                ("reserved", C.c_uint8 * 6), ("device_bytes", C.c_uint64)]
+
+
 class FgbUmiKey(C.Structure):
     _fields_ = [("bits", C.c_uint64), ("str_off", C.c_uint64), ("str_len", C.c_uint32), ("count", C.c_uint32),
                 ("first", C.c_uint32), ("dash", C.c_uint32), ("len", C.c_uint8), ("flags", C.c_uint8),
@@ -246,6 +254,7 @@ SYMBOLS = (
     "fgb_host_group_by_position", "fgb_grouper_create", "fgb_grouper_destroy", "fgb_grouper_last_error",
     "fgb_grouper_add_groups", "fgb_grouper_pending", "fgb_grouper_flush", "fgb_grouper_flush_with_ids",
     "fgb_grouper_stats", "fgb_grouper_histogram", "fgb_grouper_last_timing",
+    "fgb_sort_records", "fgb_host_sort_keys", "fgb_host_sort_verify", "fgb_sort_last_timing",
 )
 
 _lib = None
@@ -451,6 +460,17 @@ def load() -> C.CDLL:
     lib.fgb_grouper_histogram.restype = C.c_int32
     lib.fgb_grouper_last_timing.argtypes = [vp, vp]
     lib.fgb_grouper_last_timing.restype = C.c_int32
+    lib.fgb_sort_records.argtypes = [vp, C.POINTER(FgbSortOptions), C.c_char_p, C.c_size_t, vp, vp, u64, vp, u64,
+                                     C.POINTER(u64), C.POINTER(u64)]
+    lib.fgb_sort_records.restype = C.c_int32
+    lib.fgb_host_sort_keys.argtypes = [C.POINTER(FgbSortOptions), C.c_char_p, C.c_size_t, vp, vp, u64, vp,
+                                       C.POINTER(u64)]
+    lib.fgb_host_sort_keys.restype = C.c_int32
+    lib.fgb_host_sort_verify.argtypes = [C.POINTER(FgbSortOptions), C.c_char_p, C.c_size_t, vp, vp, u64,
+                                         C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
+    lib.fgb_host_sort_verify.restype = C.c_int32
+    lib.fgb_sort_last_timing.argtypes = [vp, vp]
+    lib.fgb_sort_last_timing.restype = C.c_int32
     lib.fgb_struct_size.argtypes = [C.c_uint32]
     lib.fgb_struct_size.restype = C.c_uint32
     _lib = lib

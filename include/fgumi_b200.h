@@ -979,10 +979,54 @@ fgb_status fgb_grouper_histogram(const fgb_grouper* g, int which, uint64_t* size
  * sort, tags and output stream on the host. */
 fgb_status fgb_grouper_last_timing(const fgb_grouper* g, double ms[5]);
 
+/* ---- `fgumi sort` on raw records (src/lib/sort/, src/lib/commands/sort.rs): coordinate and template-coordinate
+ * Keys (fgumi_b200/csrc/sort_keys.h, the same code on the host and the device):
+ *   coordinate: one word, (tid << 34) | ((pos + 1) << 1) | reverse, all ones for tid < 0 (the unmapped flag is not
+ *     looked at);
+ *   template-coordinate: five words compared in order -- primary (tid1, tid2, pos1 of the pair's lower end first),
+ *     secondary (pos2, inverted strands), the cell-barcode hash, tertiary (library ordinal, MI, !/A) and
+ *     name_hash << 1 | is_upper -- packed bit for bit as TemplateKey::new (inline_buffer.rs:478-520).  The library
+ *     ordinal numbers the distinct LB values of the header's @RG lines in byte order from 1 (0: no RG, an RG the
+ *     header lacks, an RG without LB).  The name and cell hashes are 64-bit FNV-1a, not the reference's ahash.
+ * The order is a stable sort by the key: records with equal keys keep their input order. */
+enum { FGB_SORT_COORDINATE = 0, FGB_SORT_TEMPLATE_COORDINATE = 1 };
+typedef struct fgb_sort_options {
+  uint32_t order;           /* FGB_SORT_*                                                                        */
+  uint32_t n_threads;       /* host threads (staging copies, host keys); 0 or 1 = the calling thread only        */
+  char cell_tag[2];         /* template-coordinate: the cell-barcode tag, "CB" as `fgumi sort` uses; "\0\0" = none */
+  uint8_t reserved[6];
+  uint64_t device_bytes;    /* device-memory budget of one sorted run; 0 = derived from cudaMemGetInfo per call  */
+} fgb_sort_options;
+/* Sorts n_records records (record i = records[rec_off[i] .. rec_off[i+1]), no block_size prefix) into `out` as
+ * [u32 block_size][record]..., the record section of a BAM: out_len = rec_off[n] - rec_off[0] + 4 n, which `cap` must
+ * hold.  Synchronous.  The records are sorted on the device in runs that fit device_bytes (keys, stable radix passes
+ * over the key words that vary, record gather); several runs are merged on the host by key, ties by run.
+ * `header_text` is the SAM header (its @RG lines give the library ordinals).  A too-small cap or bad options give
+ * FGB_ERR_INVALID_ARG; a record shorter than 32 bytes (or a descending rec_off) gives FGB_ERR_LAYOUT with
+ * *bad_record = its index.  A failing call frees whatever it allocated. */
+fgb_status fgb_sort_records(fgb_handle* h, const fgb_sort_options* opt, const char* header_text, size_t header_len,
+                            const uint8_t* records, const uint64_t* rec_off, uint64_t n_records, uint8_t* out,
+                            uint64_t cap, uint64_t* out_len, uint64_t* bad_record);
+/* The keys of fgb_sort_records on host threads (no device; there is no CPU sort): keys[5 i + w] = word w of record i
+ * (coordinate: word 0, the others 0).  Errors as fgb_sort_records. */
+fgb_status fgb_host_sort_keys(const fgb_sort_options* opt, const char* header_text, size_t header_len,
+                              const uint8_t* records, const uint64_t* rec_off, uint64_t n_records, uint64_t* keys,
+                              uint64_t* bad_record);
+/* `fgumi sort --verify` (commands/sort.rs:376-408, 700-720): the records whose key is less than the previous record's
+ * (template-coordinate: core_cmp, the first four words, inline_buffer.rs:604-618), and the index of the first of
+ * them (UINT64_MAX when there is none). */
+fgb_status fgb_host_sort_verify(const fgb_sort_options* opt, const char* header_text, size_t header_len,
+                                const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
+                                uint64_t* violations, uint64_t* first_violation, uint64_t* bad_record);
+/* Where the last fgb_sort_records on this handle spent its time, in ms, summed over its runs: [0] upload (staging
+ * copies and transfers), [1] key kernel, [2] radix passes, [3] offsets scan and record gather (CUDA events for
+ * [1]-[3]), [4] download, [5] host merge (0 for one run). */
+fgb_status fgb_sort_last_timing(const fgb_handle* h, double ms[6]);
+
 /* sizeof() of the ABI structs as this library was compiled, so a binding can check its own layout:
  * 0 fgb_caller_options, 1 fgb_filter_params, 2 fgb_submit_options, 3 fgb_raw_columns,
  * 4 fgb_raw_read, 5 fgb_batch, 6 fgb_codec_params, 7 fgb_params, 8 fgb_duplex_filter_params,
- * 9 fgb_record_columns, 10 fgb_umi_options, 11 fgb_group_options; 0 for an unknown id. */
+ * 9 fgb_record_columns, 10 fgb_umi_options, 11 fgb_group_options, 12 fgb_sort_options; 0 for an unknown id. */
 uint32_t fgb_struct_size(uint32_t id);
 
 #ifdef __cplusplus
