@@ -12,6 +12,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import sort_oracle as S       # noqa: E402
+from tests import sort_cases as SC        # noqa: E402
 from tests.bam_builder import make_record  # noqa: E402
 from tests.sort_cases import HEADER, pack, random_records  # noqa: E402
 
@@ -251,3 +252,136 @@ def test_sort_header(srt):
 def test_struct_size_of_sort_options(srt):
     from fgumi_b200 import lib as L
     assert L.load().fgb_struct_size(12) == C.sizeof(L.FgbSortOptions) == 24
+
+
+# ---- the generators and references of tests/test_sort_records_scale_gpu.py -------------------------------------------
+CASES = [(TC, b"CB"), (TC, None), (CO, None)]
+
+
+@pytest.fixture(scope="module")
+def bulk():
+    """A bulk input as the scale tests build it, at 20 000 records, with a noise lead and an unaligned bodies array."""
+    common, rare = SC.bulk_pool(3)
+    f = SC.bulk_fields(20000, 3, len(common), len(rare))
+    b, off = SC.materialize(common + rare, f, lead=77, skew=1, chunk=100_000)
+    return b, off, f
+
+
+@pytest.fixture(scope="module")
+def grid():
+    return SC.gather_grid(31)
+
+
+def test_scale_bulk_input_is_what_it_claims(bulk):
+    b, off, f = bulk
+    n = len(off) - 1
+    assert off[0] == 77 and b.ctypes.data % 4
+    recs = SC.records_of(b, off, range(n))
+    assert len(set(recs)) == n                                        # byte-unique
+    for i in (0, 1, 4567, n - 1):
+        r = recs[i]
+        assert struct.unpack_from("<ii", r, 0) == (f["tid"][i], f["pos"][i])
+        assert struct.unpack_from("<ii", r, 20) == (f["mtid"][i], f["mpos"][i])
+        assert r[14] & 0x30 == f["strand"][i]
+        assert int.from_bytes(r[9:12], "little") | int.from_bytes(r[28:32], "little") << 24 == i
+    common, rare = SC.bulk_pool(3)
+    pool = common + rare
+    for i in np.flatnonzero(f["idx"] >= len(common))[:8]:            # the rest of each record is its pool record's
+        r, p = recs[i], pool[f["idx"][i]]
+        assert len(r) == len(p) and r[32:] == p[32:] and r[12:14] == p[12:14] and r[15:20] == p[15:20]
+    assert {len(r) for r in rare} >= {65535, 65536, 65537}
+    assert max(struct.unpack_from("<H", r, 12)[0] for r in rare) == 1000
+
+
+def test_scale_serial_bytes_are_not_key_bytes(srt, bulk, grid):
+    b, off, _ = bulk
+    gb, goff = SC.pack(grid)
+    rng = np.random.default_rng(8)
+    sample = sorted(rng.choice(len(off) - 1, 2000, replace=False).tolist())
+    grid_sample = [i for i, r in enumerate(grid) if i % 4 == 0 or len(r) > 60000]
+    for bodies, rec_off, which in ((b, off, sample), (gb, goff, grid_sample)):
+        at = rec_off[:-1].astype(np.int64)
+        other = bodies.copy()
+        for k in SC.SERIAL_BYTES:
+            other[at + k] = rng.integers(0, 256, len(at), dtype=np.uint8)
+        assert not np.array_equal(other, bodies)
+        for order, cell in CASES:
+            assert np.array_equal(srt.sort_keys(HEADER, bodies, rec_off, order, cell),
+                                  srt.sort_keys(HEADER, other, rec_off, order, cell))
+            assert S.keys(SC.records_of(bodies, rec_off, which), HEADER, order, cell) == \
+                S.keys(SC.records_of(other, rec_off, which), HEADER, order, cell)
+
+
+def test_scale_numpy_coordinate_key(srt, bulk):
+    tids = SC.TIDS + [-2 ** 31, -2, 3, 2 ** 30]
+    pos = SC.POS + [-2 ** 31, -2, 2 ** 31 - 2, 2 ** 30]
+    recs = [rec(tid=t, pos=p, flags=fl) for t in tids for p in pos for fl in (0, 0x10, 0x4 | 0x10 | 0x20)]
+    b, off = SC.pack_at(recs, 3, 1)
+    want = [S.coordinate_key(r) for r in recs]
+    assert SC.coordinate_keys(b, off).tolist() == want
+    assert srt.sort_keys(HEADER, b, off, CO)[:, 0].tolist() == want
+    assert M64 in want and 0 in want and any(k >= 1 << 63 for k in want if k != M64)   # tid < 0, and the wraps
+    b, off, _ = bulk
+    assert SC.coordinate_keys(b, off).tolist() == [S.coordinate_key(r) for r in SC.records_of(b, off, range(len(off) - 1))]
+
+
+def test_scale_alignment_combinations(srt, bulk, grid):
+    """Every (source offset, output offset, length) mod 4 combination reaches the record gather."""
+    every = {(s, o, n) for s in range(4) for o in range(4) for n in range(4)}
+    b, off, _ = bulk
+    assert SC.alignments(off, SC.sorted_order(SC.coordinate_keys(b, off))) == every
+    for cell in (b"CB", None):
+        assert SC.alignments(off, SC.sorted_order(srt.sort_keys(HEADER, b, off, TC, cell))) == every
+    gb, goff = SC.pack(grid)
+    for order, cell in CASES:
+        k = S.keys(grid, HEADER, order, cell)
+        assert SC.alignments(goff, np.array(sorted(range(len(grid)), key=k.__getitem__))) == every
+
+
+def test_scale_gather_grid_shapes(grid):
+    lens = [len(r) for r in grid]
+    assert set(range(32, 401)) <= set(lens)
+    assert {65535, 65536, 65537, (1 << 20) + 3} <= set(lens)
+    n_cig = [struct.unpack_from("<H", r, 12)[0] for r in grid]
+    assert n_cig.count(65535) == 3
+    long_mc = [r for r in grid if r.find(b"MCZ") > 0 and len(r) - r.find(b"MCZ") > 100_000]
+    assert len(long_mc) == 3 and all(r.count(b"M") > 10_000 for r in long_mc)
+    assert len(set(grid)) == len(grid)
+
+
+def test_scale_references_equal_the_oracle_order(srt):
+    """A stable np.argsort of the numpy coordinate keys and a stable np.lexsort of the host key words order records as
+    the oracle's stable sort does, and the chunked expected stream is the oracle's stream (ties kept by serials)."""
+    recs = SC.stamp_serials(random_records(4000, seed=12))
+    b, off = SC.pack_at(recs, 5, 1)
+    for order, cell in CASES:
+        keys = SC.coordinate_keys(b, off) if order == CO else srt.sort_keys(HEADER, b, off, order, cell)
+        perm = SC.sorted_order(keys)
+        k = S.keys(recs, HEADER, order, cell)
+        assert perm.tolist() == sorted(range(len(recs)), key=k.__getitem__)
+        want = bytearray(S.sorted_stream(recs, HEADER, order, cell))
+        SC.assert_stream(want, b, off, perm, chunk=5000)
+        i = len(recs) // 2
+        at = int(SC.stream_offsets(off, perm)[i]) + 4 + 9            # the serial of output record i
+        want[at] ^= 1
+        with pytest.raises(AssertionError, match="output record %d " % i):
+            SC.assert_stream(want, b, off, perm, chunk=5000)
+
+
+def test_scale_run_plan():
+    """run_plan restates the run loop of fgb_sort_records; budget_for gives a first run that ends where asked."""
+    def loop(off, budget, words):
+        per, n, out, b = 68 + 8 * words, len(off) - 1, [0], 0
+        while b < n:
+            i = b + 1
+            while i < n and 2 * (off[i + 1] - off[b]) + (i + 1 - b) * (per + 4) <= budget:
+                i += 1
+            out.append(i)
+            b = i
+        return out
+    rng = np.random.default_rng(4)
+    off = [9] + (9 + np.cumsum(rng.integers(32, 700, 3000))).tolist()
+    for words in (1, 5):
+        for budget in (1, 2000, 30000, 10 ** 6, 10 ** 9):
+            assert SC.run_plan(np.array(off, np.uint64), budget, words) == loop(off, budget, words)
+        assert SC.run_plan(off, SC.budget_for(off, 1234, words), words)[1] == 1234
