@@ -150,10 +150,13 @@ def group_header(input_text: bytes, command_line: str = "fgumi_b200 group") -> b
 
 def sort_header(input_text: bytes, order: str, command_line: str = "fgumi_b200 sort") -> bytes:
     """`fgumi sort`'s output header (sort/mod.rs:72-129, raw.rs:1530-1535): the input header with one @PG chained as
-    group_header chains it, then SO / GO / SS of the @HD line removed and set again -- SO:coordinate, or SO:unsorted
-    GO:query SS:template-coordinate -- keeping VN and the other @HD fields; an @HD line is created when there is none."""
+    group_header chains it, then SO / GO / SS of the @HD line removed and set again -- SO:coordinate, SO:unsorted
+    GO:query SS:template-coordinate, or SO:queryname with SS:lexicographic or SS:natural (no GO) -- keeping VN and the
+    other @HD fields; an @HD line is created when there is none."""
     tags = {"coordinate": [("SO", "coordinate")],
-            "template-coordinate": [("SO", "unsorted"), ("GO", "query"), ("SS", "template-coordinate")]}[order]
+            "template-coordinate": [("SO", "unsorted"), ("GO", "query"), ("SS", "template-coordinate")],
+            "queryname": [("SO", "queryname"), ("SS", "lexicographic")],
+            "queryname::natural": [("SO", "queryname"), ("SS", "natural")]}[order]
     lines = group_header(input_text, command_line).decode("utf-8", "replace").rstrip("\n").split("\n")
     at = next((i for i, ln in enumerate(lines) if ln.startswith("@HD")), None)
     fields = [] if at is None else [f for f in lines[at].split("\t")[1:] if f[:3] not in ("SO:", "GO:", "SS:")]

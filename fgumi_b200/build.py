@@ -58,19 +58,19 @@ def _check_umi_kernels(ptxas_log: str) -> None:
 
 
 def _check_sort_kernels(ptxas_log: str) -> None:
-    """The sort's key kernel walks a record's CIGAR, aux block and MC string in registers, and the gather kernel copies
-    with a few words per lane: a stack frame or a spill means a source change pushed the key state into local memory,
-    and fails the build."""
+    """The sort's key kernels walk a record's CIGAR, aux block and MC string, or stream its read name, in registers,
+    and the gather kernel copies with a few words per lane: a stack frame or a spill means a source change pushed the
+    key state into local memory, and fails the build."""
     import re
     found = 0
-    for m in re.finditer(r"Function properties for (\S*sort_(?:key|gather)_kernel\S*)\n\s*(\d+) bytes stack frame, "
-                         r"(\d+) bytes spill stores", ptxas_log):
+    for m in re.finditer(r"Function properties for (\S*sort_(?:name_key|key|gather)_kernel\S*)\n\s*(\d+) bytes stack "
+                         r"frame, (\d+) bytes spill stores", ptxas_log):
         found += 1
         if int(m.group(2)) or int(m.group(3)):
             raise RuntimeError(f"fgumi_b200 build: {m.group(1)} has a {m.group(2)}-byte stack frame and spills "
                                f"{m.group(3)} bytes (expected none)")
-    if found != 3:
-        raise RuntimeError(f"fgumi_b200 build: ptxas reported {found} sort key / gather kernels, expected 3")
+    if found != 4:
+        raise RuntimeError(f"fgumi_b200 build: ptxas reported {found} sort key / gather kernels, expected 4")
 
 
 def build(force: bool = False, verbose: bool = False) -> str:

@@ -1717,6 +1717,13 @@ cudaError_t keys(const uint8_t* rec, const uint64_t* off, uint64_t base, uint32_
   return cudaGetLastError();
 }
 
+cudaError_t name_keys(const uint8_t* rec, const uint64_t* off, uint64_t base, uint32_t n, bool natural, int name_words,
+                      uint64_t* keys, uint32_t* size, unsigned long long* and_or, cudaStream_t s) {
+  if (!n) return cudaSuccess;
+  sort_name_key_kernel<<<blocks(n), kSortThreads, 0, s>>>(rec, off, base, n, natural, name_words, keys, size, and_or);
+  return cudaGetLastError();
+}
+
 cudaError_t word_gather(const uint64_t* word, const uint32_t* perm, uint32_t n, uint64_t* dst, cudaStream_t s) {
   if (!n) return cudaSuccess;
   sort_word_gather_kernel<<<blocks(n), kSortThreads, 0, s>>>(word, perm, n, dst, nullptr);

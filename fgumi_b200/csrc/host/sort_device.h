@@ -28,6 +28,9 @@ HandleInfo info(fgb_handle* h);
 // word over the run, which `and_or` must hold as (~0, 0) pairs on entry.
 cudaError_t keys(const uint8_t* rec, const uint64_t* off, uint64_t base, uint32_t n, const sortk::Ctx& ctx, int words,
                  uint64_t* keys, uint32_t* size, unsigned long long* and_or, cudaStream_t s);
+// Queryname order: name_words + 1 key words (SoA), sizes and AND / OR as keys()
+cudaError_t name_keys(const uint8_t* rec, const uint64_t* off, uint64_t base, uint32_t n, bool natural, int name_words,
+                      uint64_t* keys, uint32_t* size, unsigned long long* and_or, cudaStream_t s);
 // dst[i] = word[perm[i]]
 cudaError_t word_gather(const uint64_t* word, const uint32_t* perm, uint32_t n, uint64_t* dst, cudaStream_t s);
 cudaError_t iota(uint32_t* v, uint32_t n, cudaStream_t s);

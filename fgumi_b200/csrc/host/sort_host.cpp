@@ -1,8 +1,8 @@
-// `fgumi sort` (coordinate and template-coordinate) from raw BAM records: the header's library table, the host key
-// and verify entry points, and the driver of the device sort (fgb_sort_records): runs that fit a device budget, each
-// uploaded through page-locked staging, keyed, sorted by stable radix passes over the key words that vary and gathered
-// into a [u32 block_size][record] stream on the device; several runs are merged on the host.  The key functions are
-// ../sort_keys.h; the kernels and CUB calls sit behind sort_device.h in capi.cu.
+// `fgumi sort` (coordinate, template-coordinate and queryname) from raw BAM records: the header's library table, the
+// host key and verify entry points, and the driver of the device sort (fgb_sort_records): runs that fit a device
+// budget, each uploaded through page-locked staging, keyed, sorted by stable radix passes over the key words that vary
+// and gathered into a [u32 block_size][record] stream on the device; several runs are merged on the host.  The key
+// functions are ../sort_keys.h; the kernels and CUB calls sit behind sort_device.h in capi.cu.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -25,7 +25,8 @@ namespace {
 namespace sk = fgb::sortk;
 namespace dev = fgb::sortdev;
 
-static_assert(FGB_SORT_COORDINATE == sk::kCoordinate && FGB_SORT_TEMPLATE_COORDINATE == sk::kTemplateCoordinate,
+static_assert(FGB_SORT_COORDINATE == sk::kCoordinate && FGB_SORT_TEMPLATE_COORDINATE == sk::kTemplateCoordinate &&
+                  FGB_SORT_QUERYNAME == sk::kQueryname && FGB_SORT_QUERYNAME_NATURAL == sk::kQuerynameNatural,
               "sort orders");
 constexpr uint64_t kNone = UINT64_MAX;
 constexpr uint64_t kStageBytes = 64ull << 20;   // one page-locked staging buffer (two alternate)
@@ -59,7 +60,7 @@ Lookup library_lookup(std::string_view text) {
 }
 
 bool options_ok(const fgb_sort_options* o) {
-  if (!o || o->order > FGB_SORT_TEMPLATE_COORDINATE) return false;
+  if (!o || o->order > FGB_SORT_QUERYNAME_NATURAL) return false;
   return (o->cell_tag[0] == 0) == (o->cell_tag[1] == 0);
 }
 
@@ -73,7 +74,17 @@ sk::Ctx make_ctx(const fgb_sort_options& o, const uint8_t* bytes, const uint32_t
   return c;
 }
 
-int key_words(const fgb_sort_options& o) { return o.order == FGB_SORT_COORDINATE ? 1 : sk::kWords; }
+bool queryname(const fgb_sort_options& o) {
+  return o.order == FGB_SORT_QUERYNAME || o.order == FGB_SORT_QUERYNAME_NATURAL;
+}
+
+// Key words per record: 1 (coordinate), 5 (template-coordinate), or for queryname the name words of the longest
+// l_read_name `lrn` among the run's records plus the last word.
+int key_words(const fgb_sort_options& o, uint32_t lrn) {
+  if (queryname(o))
+    return static_cast<int>(sk::name_words(static_cast<uint8_t>(lrn), o.order == FGB_SORT_QUERYNAME_NATURAL)) + 1;
+  return o.order == FGB_SORT_COORDINATE ? 1 : sk::kWords;
+}
 
 // Each record holds its 32-byte fixed part and rec_off ascends; else *bad = the first offending record.
 bool records_ok(const uint64_t* rec_off, uint64_t n, uint64_t* bad) {
@@ -190,29 +201,42 @@ fgb_status sort_impl(fgb_handle* h, const fgb_sort_options& o, std::string_view 
   Driver d{dev::info(h), o, std::max<uint32_t>(o.n_threads, 1), {}, nullptr};
   d.s = d.hi.stream;
   double* tm = d.hi.timing;
-  const int W = key_words(o);
+  const bool qn = queryname(o), natural = o.order == FGB_SORT_QUERYNAME_NATURAL;
   cudaError_t e = cudaSetDevice(d.hi.device);
   if (e != cudaSuccess) return d.fail(e, "cudaSetDevice");
-  // runs: as many records as fit the budget (input and output bytes, keys, permutations and scan / sort scratch)
+  // runs: as many records as fit the budget (input and output bytes, keys, permutations and scan / sort scratch: 68 +
+  // 8 W bytes per record, W the run's key words)
   uint64_t budget = o.device_bytes;
   if (!budget) {
     size_t free_b = 0, total_b = 0;
     if ((e = cudaMemGetInfo(&free_b, &total_b)) != cudaSuccess) return d.fail(e, "cudaMemGetInfo");
     budget = free_b - free_b / 8 - std::min<uint64_t>(free_b / 8, 512ull << 20);
   }
-  const uint64_t per_record = 68 + 8ull * W;
+  auto lrn = [&](uint64_t i) -> uint32_t { return qn ? records[rec_off[i] + 8] : 0; };   // l_read_name
   std::vector<uint64_t> run_begin{0};
-  uint64_t max_n = 0, max_bytes = 0;
+  std::vector<int> run_words;
+  uint64_t max_n = 0, max_bytes = 0, max_cells = 0;
+  int max_words = 0;
   for (uint64_t b = 0; b < n;) {
     uint64_t i = b + 1;   // at least one record per run
-    while (i < n && i - b < INT32_MAX &&
-           2 * (rec_off[i + 1] - rec_off[b]) + (i + 1 - b) * (per_record + 4) <= budget) ++i;
+    uint32_t l = lrn(b);
+    while (i < n && i - b < INT32_MAX) {
+      const uint32_t li = std::max(l, lrn(i));
+      if (2 * (rec_off[i + 1] - rec_off[b]) + (i + 1 - b) * (68 + 8ull * key_words(o, li) + 4) > budget) break;
+      l = li;
+      ++i;
+    }
+    const int words = key_words(o, l);
     max_n = std::max(max_n, i - b);
     max_bytes = std::max(max_bytes, rec_off[i] - rec_off[b]);
+    max_cells = std::max(max_cells, static_cast<uint64_t>(words) * (i - b));
+    max_words = std::max(max_words, words);
     run_begin.push_back(i);
+    run_words.push_back(words);
     b = i;
   }
   const uint64_t n_runs = run_begin.size() - 1;
+  const bool merge_keys = n_runs > 1 && !qn;   // the queryname merge compares the records themselves
   // buffers for the largest run
   const Lookup l = library_lookup(header);
   uint8_t *d_rec, *d_out, *d_rg, *d_temp;
@@ -225,13 +249,13 @@ fgb_status sort_impl(fgb_handle* h, const fgb_sort_options& o, std::string_view 
       (e = dev::out_offsets(nullptr, &t_scan, nullptr, nullptr, mn, nullptr, nullptr, d.s)) != cudaSuccess)
     return d.fail(e, "CUB temp storage");
   if ((e = d.r.alloc(&d_rec, max_bytes + 16)) != cudaSuccess || (e = d.r.alloc(&d_out, max_bytes + 4 * max_n)) ||
-      (e = d.r.alloc(&d_off, max_n + 1)) || (e = d.r.alloc(&d_keys, W * max_n)) ||
+      (e = d.r.alloc(&d_off, max_n + 1)) || (e = d.r.alloc(&d_keys, max_cells)) ||
       (e = d.r.alloc(&d_ktmp[0], max_n)) || (e = d.r.alloc(&d_ktmp[1], max_n)) ||
       (e = d.r.alloc(&d_osize, max_n + 1)) || (e = d.r.alloc(&d_ooff, max_n + 1)) || (e = d.r.alloc(&d_size, max_n)) ||
       (e = d.r.alloc(&d_perm[0], max_n)) || (e = d.r.alloc(&d_perm[1], max_n)) ||
       (e = d.r.alloc(&d_rg, l.bytes.size())) || (e = d.r.alloc(&d_rgoff, l.off.size())) ||
-      (e = d.r.alloc(&d_rglib, l.lib.size())) || (e = d.r.alloc(&d_andor, 2 * W)) ||
-      (e = d.r.alloc(&d_temp, std::max(t_sort, t_scan) + 16)) || (n_runs > 1 && (e = d.r.alloc(&d_rows, W * max_n))))
+      (e = d.r.alloc(&d_rglib, l.lib.size())) || (e = d.r.alloc(&d_andor, 2 * max_words)) ||
+      (e = d.r.alloc(&d_temp, std::max(t_sort, t_scan) + 16)) || (merge_keys && (e = d.r.alloc(&d_rows, max_cells))))
     return d.fail(e, "cudaMalloc");
   const uint64_t stage = std::min<uint64_t>(kStageBytes, std::max(max_bytes + 4 * max_n, (max_n + 1) * 8));
   for (int b = 0; b < 2; ++b) {
@@ -249,25 +273,26 @@ fgb_status sort_impl(fgb_handle* h, const fgb_sort_options& o, std::string_view 
   const sk::Ctx ctx = make_ctx(o, d_rg, d_rgoff, d_rglib, static_cast<uint32_t>(l.lib.size()));
   // several runs: each run's sorted stream and its keys in sorted order (row-major) come back for the merge
   std::vector<uint8_t> run_stream;
-  std::vector<std::vector<uint64_t>> run_keys(n_runs > 1 ? n_runs : 0);
+  std::vector<std::vector<uint64_t>> run_keys(merge_keys ? n_runs : 0);
   if (n_runs > 1) run_stream.resize(rec_off[n] - rec_off[0] + 4 * n);
+  std::vector<unsigned long long> init(2 * max_words), and_or(2 * max_words);
+  for (int w = 0; w < max_words; ++w) { init[2 * w] = ~0ull; init[2 * w + 1] = 0; }
   for (uint64_t x = 0; x < n_runs; ++x) {
     const uint64_t b = run_begin[x], nr64 = run_begin[x + 1] - b;
     const uint32_t nr = static_cast<uint32_t>(nr64);
+    const int W = run_words[x];
     const uint64_t base = rec_off[b], bytes = rec_off[b + nr64] - base, out_at = base - rec_off[0] + 4 * b;
     auto t0 = std::chrono::steady_clock::now();
     if ((e = d.upload(d_rec, records + base, bytes)) != cudaSuccess ||
         (e = d.upload(reinterpret_cast<uint8_t*>(d_off), reinterpret_cast<const uint8_t*>(rec_off + b), (nr64 + 1) * 8)))
       return d.fail(e, "upload");
     tm[0] += ms_since(t0);
-    unsigned long long init[2 * sk::kWords];
-    for (int w = 0; w < W; ++w) { init[2 * w] = ~0ull; init[2 * w + 1] = 0; }
-    unsigned long long and_or[2 * sk::kWords];
-    if ((e = cudaMemcpyAsync(d_andor, init, 16 * W, cudaMemcpyHostToDevice, d.s)) ||
+    if ((e = cudaMemcpyAsync(d_andor, init.data(), 16 * W, cudaMemcpyHostToDevice, d.s)) ||
         (e = cudaEventRecord(d.r.ev[0], d.s)) ||
-        (e = dev::keys(d_rec, d_off, base, nr, ctx, W, d_keys, d_size, d_andor, d.s)) ||
+        (e = qn ? dev::name_keys(d_rec, d_off, base, nr, natural, W - 1, d_keys, d_size, d_andor, d.s)
+                : dev::keys(d_rec, d_off, base, nr, ctx, W, d_keys, d_size, d_andor, d.s)) ||
         (e = cudaEventRecord(d.r.ev[1], d.s)) ||
-        (e = cudaMemcpyAsync(and_or, d_andor, 16 * W, cudaMemcpyDeviceToHost, d.s)) ||
+        (e = cudaMemcpyAsync(and_or.data(), d_andor, 16 * W, cudaMemcpyDeviceToHost, d.s)) ||
         (e = cudaStreamSynchronize(d.s)))
       return d.fail(e, "key kernel");
     // LSD over the words, last first, skipping constant ones and sorting only the bits that vary
@@ -293,7 +318,7 @@ fgb_status sort_impl(fgb_handle* h, const fgb_sort_options& o, std::string_view 
     if ((e = cudaEventRecord(d.r.ev[3], d.s)) ||
         (e = dev::out_offsets(d_temp, &tb, d_size, perm, nr, d_osize, d_ooff, d.s)) ||
         (e = dev::gather(d_rec, d_off, base, perm, d_ooff, nr, d_out, d.hi.sm_count, d.s)) ||
-        (n_runs > 1 && (e = dev::key_rows(d_keys, perm, nr, W, d_rows, d.s))) ||
+        (merge_keys && (e = dev::key_rows(d_keys, perm, nr, W, d_rows, d.s))) ||
         (e = cudaEventRecord(d.r.ev[4], d.s)) || (e = cudaStreamSynchronize(d.s)))
       return d.fail(e, "gather");
     float k_ms = 0, s_ms = 0, g_ms = 0;
@@ -305,7 +330,7 @@ fgb_status sort_impl(fgb_handle* h, const fgb_sort_options& o, std::string_view 
     const uint64_t out_bytes = bytes + 4 * nr64;
     if ((e = d.download((n_runs > 1 ? run_stream.data() : out) + out_at, d_out, out_bytes)))
       return d.fail(e, "download");
-    if (n_runs > 1) {
+    if (merge_keys) {
       run_keys[x].resize(W * nr64);
       if ((e = cudaMemcpy(run_keys[x].data(), d_rows, W * nr64 * 8, cudaMemcpyDeviceToHost)))
         return d.fail(e, "download");
@@ -313,11 +338,21 @@ fgb_status sort_impl(fgb_handle* h, const fgb_sort_options& o, std::string_view 
     tm[4] += ms_since(t0);
   }
   if (n_runs <= 1) return FGB_OK;
-  // k-way merge by the key words, ties by run index: a binary heap of run heads
+  // k-way merge by the key words, ties by run index: a binary heap of run heads.  Queryname runs are merged with the
+  // reference comparator on the head records themselves, not with the encoded keys, so that the tests comparing many
+  // runs with one run also check the encoding against the comparator.
   const auto t0 = std::chrono::steady_clock::now();
+  const int W = run_words[0];
   std::vector<uint64_t> pos(n_runs, 0), cur(n_runs);
   for (uint64_t x = 0; x < n_runs; ++x) cur[x] = rec_off[run_begin[x]] - rec_off[0] + 4 * run_begin[x];
   auto after = [&](uint64_t a, uint64_t b) {   // heap order: true when run a's head goes after run b's
+    if (qn) {
+      uint32_t la, lb;
+      std::memcpy(&la, run_stream.data() + cur[a], 4);
+      std::memcpy(&lb, run_stream.data() + cur[b], 4);
+      const int c = sk::queryname_cmp(run_stream.data() + cur[a] + 4, la, run_stream.data() + cur[b] + 4, lb, natural);
+      return c ? c > 0 : a > b;
+    }
     const uint64_t* ka = run_keys[a].data() + W * pos[a];
     const uint64_t* kb = run_keys[b].data() + W * pos[b];
     for (int w = 0; w < W; ++w)
@@ -350,7 +385,7 @@ extern "C" {
 fgb_status fgb_host_sort_keys(const fgb_sort_options* opt, const char* header_text, size_t header_len,
                               const uint8_t* records, const uint64_t* rec_off, uint64_t n_records, uint64_t* keys,
                               uint64_t* bad_record) {
-  if (!args_ok(opt, header_text, header_len, records, rec_off, n_records) || (n_records && !keys))
+  if (!args_ok(opt, header_text, header_len, records, rec_off, n_records) || queryname(*opt) || (n_records && !keys))
     return FGB_ERR_INVALID_ARG;
   if (bad_record) *bad_record = kNone;
   if (!records_ok(rec_off, n_records, bad_record)) return FGB_ERR_LAYOUT;
@@ -369,6 +404,30 @@ fgb_status fgb_host_sort_verify(const fgb_sort_options* opt, const char* header_
     return FGB_ERR_INVALID_ARG;
   if (bad_record) *bad_record = kNone;
   if (!records_ok(rec_off, n_records, bad_record)) return FGB_ERR_LAYOUT;
+  if (queryname(*opt)) {   // the full key: the name comparator, then the flag order
+    const bool natural = opt->order == FGB_SORT_QUERYNAME_NATURAL;
+    const uint64_t t = std::max<uint32_t>(opt->n_threads, 1);
+    std::vector<uint64_t> v(t, 0), first(t, kNone);
+    try {
+      fgb_umi::parallel_for(t, opt->n_threads, [&](uint64_t w) {
+        for (uint64_t i = std::max<uint64_t>(n_records * w / t, 1), e = n_records * (w + 1) / t; i < e; ++i)
+          if (sk::queryname_cmp(records + rec_off[i], rec_off[i + 1] - rec_off[i], records + rec_off[i - 1],
+                                rec_off[i] - rec_off[i - 1], natural) < 0) {
+            ++v[w];
+            if (first[w] == kNone) first[w] = i;
+          }
+      });
+    } catch (const std::exception&) {
+      return FGB_ERR_NOMEM;
+    }
+    *violations = 0;
+    *first_violation = kNone;
+    for (uint64_t w = 0; w < t; ++w) {
+      *violations += v[w];
+      *first_violation = std::min(*first_violation, first[w]);
+    }
+    return FGB_OK;
+  }
   try {
     std::vector<uint64_t> k(sk::kWords * n_records);
     host_keys(*opt, std::string_view(header_text ? header_text : "", header_len), records, rec_off, n_records, k.data());
@@ -387,6 +446,20 @@ fgb_status fgb_host_sort_verify(const fgb_sort_options* opt, const char* header_
   } catch (const std::exception&) {
     return FGB_ERR_NOMEM;
   }
+  return FGB_OK;
+}
+
+fgb_status fgb_host_sort_name_key(const fgb_sort_options* opt, const uint8_t* record, uint64_t len, uint64_t* words,
+                                  uint32_t cap, uint32_t* n_words) {
+  if (!options_ok(opt) || !queryname(*opt) || !record || !n_words) return FGB_ERR_INVALID_ARG;
+  if (len < 32) return FGB_ERR_LAYOUT;
+  const int W = key_words(*opt, record[8]);
+  *n_words = static_cast<uint32_t>(W);
+  if (cap < static_cast<uint32_t>(W) || !words) return FGB_ERR_INVALID_ARG;
+  sk::NameEncoder enc;
+  enc.init(record, len, opt->order == FGB_SORT_QUERYNAME_NATURAL);
+  for (int w = 0; w + 1 < W; ++w) words[w] = enc.word();
+  words[W - 1] = sk::name_last_word(enc, record);
   return FGB_OK;
 }
 

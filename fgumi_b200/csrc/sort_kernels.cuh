@@ -1,4 +1,4 @@
-// `fgumi sort` on the device: the key kernel, the word gather between LSD passes and the record gather.  The stable
+// `fgumi sort` on the device: the key kernels, the word gather between LSD passes and the record gather.  The stable
 // sort itself is CUB's radix sort, one pass per key word that varies (driven by host/sort_host.cpp through the
 // launchers in capi.cu).
 #pragma once
@@ -49,6 +49,47 @@ __global__ void __launch_bounds__(kSortThreads) sort_key_kernel(const uint8_t* _
     for (int w = 0; w < W; ++w) {
       atomicAnd(and_or + 2 * w, static_cast<unsigned long long>(a[w]));
       atomicOr(and_or + 2 * w + 1, static_cast<unsigned long long>(o[w]));
+    }
+  }
+}
+
+// Queryname order, one record per thread: its W name words and its last word (sort_keys.h NameEncoder) as SoA
+// (keys[w * n + i], w = 0..W), its size, and the AND / OR of each of the W + 1 words over the run, as sort_key_kernel.
+// The encoder streams the name from the record into one word at a time; the host has chosen W for the run's longest
+// name, so every thread runs the same W + 1 steps and the warp reductions stay converged.
+__global__ void __launch_bounds__(kSortThreads) sort_name_key_kernel(const uint8_t* __restrict__ rec,
+                                                                     const uint64_t* __restrict__ off, uint64_t base,
+                                                                     uint32_t n, bool natural, int W,
+                                                                     uint64_t* __restrict__ keys,
+                                                                     uint32_t* __restrict__ size,
+                                                                     unsigned long long* __restrict__ and_or) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool live = i < n;
+  const uint8_t* r = nullptr;
+  sortk::NameEncoder enc;
+  if (live) {
+    const uint64_t b = off[i], e = off[i + 1];
+    r = rec + (b - base);
+    enc.init(r, e - b, natural);
+    size[i] = static_cast<uint32_t>(e - b);
+  } else {
+    enc.init_empty();
+  }
+  for (int w = 0; w <= W; ++w) {
+    uint64_t a = ~0ull, o = 0;
+    if (live) {
+      const uint64_t k = w < W ? enc.word() : sortk::name_last_word(enc, r);
+      keys[static_cast<uint64_t>(w) * n + i] = k;
+      a = o = k;
+    }
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) {
+      a &= __shfl_xor_sync(0xffffffffu, a, s);
+      o |= __shfl_xor_sync(0xffffffffu, o, s);
+    }
+    if ((threadIdx.x & 31) == 0) {
+      atomicAnd(and_or + 2 * w, static_cast<unsigned long long>(a));
+      atomicOr(and_or + 2 * w + 1, static_cast<unsigned long long>(o));
     }
   }
 }

@@ -1,7 +1,8 @@
-// Sort keys of `fgumi sort` (coordinate and template-coordinate) from raw BAM records, written once for the host and
-// the device (FGB_HD): the key kernel (sort_kernels.cuh) runs one record per thread, fgb_host_sort_keys and
-// fgb_host_sort_verify run the very same functions on host threads, and the CPU tests compare both with
-// oracle/sort_oracle.py.  Citations are relative to the fgumi 0.2.0 source tree:
+// Sort keys of `fgumi sort` (coordinate, template-coordinate and queryname) from raw BAM records, written once for the
+// host and the device (FGB_HD): the key kernels (sort_kernels.cuh) run one record per thread, fgb_host_sort_keys,
+// fgb_host_sort_name_key and fgb_host_sort_verify run the very same functions on host threads, and the CPU tests
+// compare both with oracle/sort_oracle.py (queryname: tests/queryname_oracle.py).  Citations are relative to the
+// fgumi 0.2.0 source tree:
 //   inline_buffer.rs  src/lib/sort/inline_buffer.rs         (PackedCoordinateKey, TemplateKey, core_cmp)
 //   raw.rs            src/lib/sort/raw.rs                   (LibraryLookup, extract_template_key_inline)
 //   tags.rs           crates/fgumi-raw-bam/src/tags.rs      (parse_mi_bytes, extract_template_aux_tags)
@@ -29,8 +30,9 @@
 namespace fgb {
 namespace sortk {
 
-enum : uint32_t { kCoordinate = 0, kTemplateCoordinate = 1 };
+enum : uint32_t { kCoordinate = 0, kTemplateCoordinate = 1, kQueryname = 2, kQuerynameNatural = 3 };
 constexpr int kWords = 5;   // primary, secondary, cb_hash, tertiary, name_hash_upper
+constexpr int kNameWordsMax = 64;   // queryname: a 254-byte name encodes to at most 2 * 254 + 1 bytes (natural)
 constexpr int32_t kI32Max = 2147483647;
 
 // What the key functions need beyond the record: the header's RG -> library table (IDs sorted bytewise, so a
@@ -371,6 +373,135 @@ FGB_HD bool record_key(const uint8_t* r, uint64_t n, const Ctx& c, uint64_t k[kW
   if (c.order == kCoordinate) k[0] = coordinate_key(r);
   else template_key(r, n, c, k);
   return true;
+}
+
+// ---- queryname (keys.rs:338-363, 446-456, 495-628; natural_compare_nul in crates/fgumi-raw-bam/src/sort.rs:181-238) --
+// The key of a record is a byte string E, zero-padded to W big-endian words, then one word
+// (len(E) << 16) | queryname_flag_order(flag).  Comparing the W + 1 words in order is exactly the reference comparator
+// (DESIGN.md section 10 has the argument):
+//   lexicographic: E = the name bytes, embedded NULs included;
+//   natural:       E = the name cut at its first NUL, each maximal run of ASCII digits replaced by 0x30, the count of
+//                  its significant digits (leading zeros stripped) and those digits; other bytes copied.
+
+// queryname_flag_order (keys.rs:361-363): R1 / R2, then secondary, then supplementary
+FGB_HD uint32_t queryname_flag_order(uint16_t f) {
+  return ((f & 0xc0u) << 8) | ((f & 0x100u) << 3) | ((f & 0x800u) >> 3);
+}
+
+// extract_raw_name_and_flags (keys.rs:450-456): bam[32 .. 32 + l_read_name - 1] when that fits the record, else empty
+FGB_HD uint32_t name_length(const uint8_t* r, uint64_t n) {
+  const uint32_t l = r[8] ? r[8] - 1u : 0;
+  return l > 0 && 32 + static_cast<uint64_t>(l) <= n ? l : 0;
+}
+
+// The name words W of a record whose l_read_name byte is `lrn`: E has at most lrn - 1 bytes (natural: 2 (lrn - 1) + 1,
+// every other byte a one-digit run).  A run uses the largest W of its records.
+FGB_HD uint32_t name_words(uint8_t lrn, bool natural) {
+  const uint32_t l = lrn ? lrn - 1u : 0;
+  const uint32_t e = natural && l ? 2 * l + 1 : l;
+  return (e + 7) / 8;
+}
+
+// E one byte at a time, read straight from the record (no copy of the name): next() is the next byte, or -1 after the
+// last; `len` counts the bytes returned.
+struct NameEncoder {
+  const uint8_t* s;
+  uint32_t n, i, run_end, len;
+  uint8_t phase;   // natural: 0 between tokens, 1 the count byte is next, 2 digits [i, run_end) are next
+  bool natural;
+
+  FGB_HD void init(const uint8_t* r, uint64_t rn, bool nat) {
+    s = r + 32;
+    n = name_length(r, rn);
+    if (nat) n = static_cast<uint32_t>(find_nul(s, n));   // natural_compare_nul stops at the first NUL
+    i = run_end = len = 0;
+    phase = 0;
+    natural = nat;
+  }
+  FGB_HD void init_empty() { s = nullptr; n = i = run_end = len = 0; phase = 0; natural = false; }
+
+  FGB_HD int next() {
+    if (phase == 2) {
+      if (i < run_end) { ++len; return s[i++]; }
+      phase = 0;
+    }
+    if (phase == 1) { phase = 2; ++len; return static_cast<int>(run_end - i); }
+    if (i >= n) return -1;
+    const uint8_t c = s[i];
+    ++len;
+    if (!natural || !is_digit(c)) { ++i; return c; }
+    uint32_t e = i;
+    while (e < n && is_digit(s[e])) ++e;
+    while (i < e && s[i] == '0') ++i;
+    run_end = e;
+    phase = 1;
+    return 0x30;
+  }
+
+  // the next big-endian word of E, zero-padded past its end
+  FGB_HD uint64_t word() {
+    uint64_t w = 0;
+    for (int b = 0; b < 8; ++b) {
+      const int c = next();
+      w = (w << 8) | static_cast<uint64_t>(c < 0 ? 0 : c);
+    }
+    return w;
+  }
+};
+
+// The last key word, once all W name words have been taken from `e`
+FGB_HD uint64_t name_last_word(const NameEncoder& e, const uint8_t* r) {
+  return (static_cast<uint64_t>(e.len) << 16) | queryname_flag_order(ld16(r + 14));
+}
+
+// The reference comparator on two records (the host merge and --verify): the lexicographic byte compare of
+// RawQuerynameLexKey::cmp (keys.rs:624-628) or natural_compare_nul, then the flag order.  Negative, 0 or positive.
+FGB_HD int nul_at(const uint8_t* s, uint32_t n, uint32_t p) { return p < n ? s[p] : 0; }
+
+FGB_HD int natural_compare_nul(const uint8_t* a, uint32_t na, const uint8_t* b, uint32_t nb) {
+  // sort.rs:181-238 over names cut at their first NUL; index n reads as the terminating NUL
+  uint32_t pa = 0, pb = 0;
+  while (nul_at(a, na, pa) && nul_at(b, nb, pb)) {
+    const int ca = nul_at(a, na, pa), cb = nul_at(b, nb, pb);
+    if (!is_digit(static_cast<uint8_t>(ca)) || !is_digit(static_cast<uint8_t>(cb))) {
+      if (ca != cb) return ca - cb;
+      ++pa; ++pb;
+    } else {
+      while (nul_at(a, na, pa) == '0') ++pa;
+      while (nul_at(b, nb, pb) == '0') ++pb;
+      while (is_digit(static_cast<uint8_t>(nul_at(a, na, pa))) && nul_at(a, na, pa) == nul_at(b, nb, pb)) { ++pa; ++pb; }
+      const bool a_digit = is_digit(static_cast<uint8_t>(nul_at(a, na, pa)));
+      const bool b_digit = is_digit(static_cast<uint8_t>(nul_at(b, nb, pb)));
+      const int diff = nul_at(a, na, pa) - nul_at(b, nb, pb);
+      if (a_digit && b_digit) { ++pa; ++pb; }
+      while (is_digit(static_cast<uint8_t>(nul_at(a, na, pa))) && is_digit(static_cast<uint8_t>(nul_at(b, nb, pb)))) {
+        ++pa; ++pb;
+      }
+      if (is_digit(static_cast<uint8_t>(nul_at(a, na, pa)))) return 1;
+      if (is_digit(static_cast<uint8_t>(nul_at(b, nb, pb)))) return -1;
+      if (diff) return diff;
+    }
+  }
+  if (nul_at(a, na, pa)) return 1;
+  if (nul_at(b, nb, pb)) return -1;
+  return 0;
+}
+
+FGB_HD int queryname_cmp(const uint8_t* a, uint64_t na, const uint8_t* b, uint64_t nb, bool natural) {
+  uint32_t la = name_length(a, na), lb = name_length(b, nb);
+  int c = 0;
+  if (natural) {
+    la = static_cast<uint32_t>(find_nul(a + 32, la));
+    lb = static_cast<uint32_t>(find_nul(b + 32, lb));
+    c = natural_compare_nul(a + 32, la, b + 32, lb);
+  } else {
+    const uint32_t m = la < lb ? la : lb;
+    for (uint32_t i = 0; i < m && !c; ++i) c = static_cast<int>(a[32 + i]) - static_cast<int>(b[32 + i]);
+    if (!c) c = la < lb ? -1 : la > lb ? 1 : 0;
+  }
+  if (c) return c;
+  const uint32_t fa = queryname_flag_order(ld16(a + 14)), fb = queryname_flag_order(ld16(b + 14));
+  return fa < fb ? -1 : fa > fb ? 1 : 0;
 }
 
 }  // namespace sortk

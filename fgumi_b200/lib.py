@@ -210,7 +210,7 @@ GROUP_STAT_NAMES = ("total_records", "accepted_records", "discarded_non_pf", "di
 FGB_GROUP_HIST_FAMILY, FGB_GROUP_HIST_POSITION = 0, 1
 
 
-FGB_SORT_COORDINATE, FGB_SORT_TEMPLATE_COORDINATE = 0, 1
+FGB_SORT_COORDINATE, FGB_SORT_TEMPLATE_COORDINATE, FGB_SORT_QUERYNAME, FGB_SORT_QUERYNAME_NATURAL = 0, 1, 2, 3
 
 
 class FgbSortOptions(C.Structure):
@@ -254,7 +254,7 @@ SYMBOLS = (
     "fgb_host_group_by_position", "fgb_grouper_create", "fgb_grouper_destroy", "fgb_grouper_last_error",
     "fgb_grouper_add_groups", "fgb_grouper_pending", "fgb_grouper_flush", "fgb_grouper_flush_with_ids",
     "fgb_grouper_stats", "fgb_grouper_histogram", "fgb_grouper_last_timing",
-    "fgb_sort_records", "fgb_host_sort_keys", "fgb_host_sort_verify", "fgb_sort_last_timing",
+    "fgb_sort_records", "fgb_host_sort_keys", "fgb_host_sort_verify", "fgb_sort_last_timing", "fgb_host_sort_name_key",
 )
 
 _lib = None
@@ -469,6 +469,8 @@ def load() -> C.CDLL:
     lib.fgb_host_sort_verify.argtypes = [C.POINTER(FgbSortOptions), C.c_char_p, C.c_size_t, vp, vp, u64,
                                          C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
     lib.fgb_host_sort_verify.restype = C.c_int32
+    lib.fgb_host_sort_name_key.argtypes = [C.POINTER(FgbSortOptions), vp, u64, vp, u32, C.POINTER(u32)]
+    lib.fgb_host_sort_name_key.restype = C.c_int32
     lib.fgb_sort_last_timing.argtypes = [vp, vp]
     lib.fgb_sort_last_timing.restype = C.c_int32
     lib.fgb_struct_size.argtypes = [C.c_uint32]

@@ -1,5 +1,6 @@
-"""`fgumi sort` on raw BAM records: coordinate and template-coordinate order, keyed, radix-sorted and gathered on the
-device (fgb_sort_records), with the same keys and `--verify` on the host (fgb_host_sort_keys / fgb_host_sort_verify).
+"""`fgumi sort` on raw BAM records: coordinate, template-coordinate and queryname order (lexicographic and natural),
+keyed, radix-sorted and gathered on the device (fgb_sort_records), with the same keys and `--verify` on the host
+(fgb_host_sort_keys, fgb_host_sort_name_key, fgb_host_sort_verify).
 
     s = RecordSorter(device=0, order="template-coordinate")
     stream = s.sort(header_text, bodies, rec_off)     # bytearray: [u32 block_size][record]..., stable by the key
@@ -16,15 +17,18 @@ import numpy as np
 
 from . import lib as _l
 
-ORDERS = {"coordinate": _l.FGB_SORT_COORDINATE, "template-coordinate": _l.FGB_SORT_TEMPLATE_COORDINATE}
+ORDERS = {"coordinate": _l.FGB_SORT_COORDINATE, "template-coordinate": _l.FGB_SORT_TEMPLATE_COORDINATE,
+          "queryname": _l.FGB_SORT_QUERYNAME, "queryname::natural": _l.FGB_SORT_QUERYNAME_NATURAL}
+NAME_KEY_WORDS = 65                                  # queryname: at most 64 name words and the last word
 TIMING_NAMES = ("upload_ms", "key_kernel_ms", "sort_ms", "gather_ms", "download_ms", "merge_ms")
 
 
 def options(order: str = "template-coordinate", cell_tag: Optional[bytes] = b"CB", device_bytes: int = 0,
             n_threads: Optional[int] = None) -> _l.FgbSortOptions:
-    """fgb_sort_options; cell_tag None = no cell barcode in the template-coordinate key."""
+    """fgb_sort_options; cell_tag None = no cell barcode in the template-coordinate key (the other orders ignore
+    it)."""
     if order not in ORDERS:
-        raise ValueError(f"unknown sort order {order!r} (coordinate, template-coordinate)")
+        raise ValueError(f"unknown sort order {order!r} ({', '.join(ORDERS)})")
     if cell_tag is not None and len(cell_tag) != 2:
         raise ValueError("cell_tag must be two characters")
     threads = min(os.cpu_count() or 1, 16) if n_threads is None else n_threads
@@ -46,7 +50,8 @@ def _layout_error(st: int, bad: int, where: str):
 
 def sort_keys(header_text: bytes, bodies, rec_off, order: str = "template-coordinate",
               cell_tag: Optional[bytes] = b"CB", n_threads: Optional[int] = None) -> np.ndarray:
-    """The sort keys of every record as uint64[n, 5] (coordinate: column 0), from the code the key kernel runs."""
+    """The sort keys of every record as uint64[n, 5] (coordinate: column 0), from the code the key kernel runs.
+    Coordinate and template-coordinate only: queryname keys are name_key's."""
     lib = _l.load()
     b, off = _arrays(bodies, rec_off)
     n = len(off) - 1
@@ -58,6 +63,24 @@ def sort_keys(header_text: bytes, bodies, rec_off, order: str = "template-coordi
     if st != _l.FGB_OK:
         _layout_error(st, bad.value, "fgb_host_sort_keys")
     return keys[:n]
+
+
+def name_key(record: bytes, order: str = "queryname") -> Tuple[int, ...]:
+    """The queryname key words of one record (no block_size prefix) from the code the key kernel runs: its name words,
+    zero-padded to 64 as they would be in a run with longer names, then the last word (len(E) << 16 | flag order).
+    Tuples of any two records compare as the device sorts them."""
+    if order not in ("queryname", "queryname::natural"):
+        raise ValueError(f"name_key takes a queryname order, not {order!r}")
+    rec = np.frombuffer(bytes(record) or b"\0", np.uint8)
+    words = np.zeros(NAME_KEY_WORDS, np.uint64)
+    n = C.c_uint32()
+    o = options(order, None, 0, 1)
+    st = _l.load().fgb_host_sort_name_key(C.byref(o), rec.ctypes.data, len(record), words.ctypes.data,
+                                          NAME_KEY_WORDS, C.byref(n))
+    if st != _l.FGB_OK:
+        raise _l.FgbError(st, "fgb_host_sort_name_key")
+    k = n.value - 1
+    return tuple(int(w) for w in words[:k]) + (0,) * (NAME_KEY_WORDS - 1 - k) + (int(words[k]),)
 
 
 def verify(header_text: bytes, bodies, rec_off, order: str = "template-coordinate",

@@ -979,17 +979,28 @@ fgb_status fgb_grouper_histogram(const fgb_grouper* g, int which, uint64_t* size
  * sort, tags and output stream on the host. */
 fgb_status fgb_grouper_last_timing(const fgb_grouper* g, double ms[5]);
 
-/* ---- `fgumi sort` on raw records (src/lib/sort/, src/lib/commands/sort.rs): coordinate and template-coordinate
- * Keys (fgumi_b200/csrc/sort_keys.h, the same code on the host and the device):
+/* ---- `fgumi sort` on raw records (src/lib/sort/, src/lib/commands/sort.rs): coordinate, template-coordinate and
+ * queryname.  Keys (fgumi_b200/csrc/sort_keys.h, the same code on the host and the device):
  *   coordinate: one word, (tid << 34) | ((pos + 1) << 1) | reverse, all ones for tid < 0 (the unmapped flag is not
  *     looked at);
  *   template-coordinate: five words compared in order -- primary (tid1, tid2, pos1 of the pair's lower end first),
  *     secondary (pos2, inverted strands), the cell-barcode hash, tertiary (library ordinal, MI, !/A) and
  *     name_hash << 1 | is_upper -- packed bit for bit as TemplateKey::new (inline_buffer.rs:478-520).  The library
  *     ordinal numbers the distinct LB values of the header's @RG lines in byte order from 1 (0: no RG, an RG the
- *     header lacks, an RG without LB).  The name and cell hashes are 64-bit FNV-1a, not the reference's ahash.
+ *     header lacks, an RG without LB).  The name and cell hashes are 64-bit FNV-1a, not the reference's ahash;
+ *   queryname (`--order queryname`, lexicographic) and queryname natural (`--order queryname::natural`): the read name
+ *     (empty when l_read_name < 2 or the name runs past the record), then
+ *     queryname_flag_order(flag) = ((f & 0xc0) << 8) | ((f & 0x100) << 3) | ((f & 0x800) >> 3) (keys.rs:338-363).
+ *     Lexicographic compares the name bytes, embedded NULs included; natural is natural_compare_nul (the name cut at
+ *     its first NUL; digit runs compare by value, so "01" and "1" are equal).  Encoded exactly as W big-endian words
+ *     of a byte string E plus the word (len(E) << 16) | flag order (fgb_host_sort_name_key); cell_tag is ignored.
  * The order is a stable sort by the key: records with equal keys keep their input order. */
-enum { FGB_SORT_COORDINATE = 0, FGB_SORT_TEMPLATE_COORDINATE = 1 };
+enum {
+  FGB_SORT_COORDINATE = 0,
+  FGB_SORT_TEMPLATE_COORDINATE = 1,
+  FGB_SORT_QUERYNAME = 2,           /* SO:queryname SS:lexicographic */
+  FGB_SORT_QUERYNAME_NATURAL = 3    /* SO:queryname SS:natural       */
+};
 typedef struct fgb_sort_options {
   uint32_t order;           /* FGB_SORT_*                                                                        */
   uint32_t n_threads;       /* host threads (staging copies, host keys); 0 or 1 = the calling thread only        */
@@ -1008,13 +1019,21 @@ fgb_status fgb_sort_records(fgb_handle* h, const fgb_sort_options* opt, const ch
                             const uint8_t* records, const uint64_t* rec_off, uint64_t n_records, uint8_t* out,
                             uint64_t cap, uint64_t* out_len, uint64_t* bad_record);
 /* The keys of fgb_sort_records on host threads (no device; there is no CPU sort): keys[5 i + w] = word w of record i
- * (coordinate: word 0, the others 0).  Errors as fgb_sort_records. */
+ * (coordinate: word 0, the others 0).  Errors as fgb_sort_records; the queryname orders, whose keys do not fit five
+ * words, give FGB_ERR_INVALID_ARG (their keys come from fgb_host_sort_name_key). */
 fgb_status fgb_host_sort_keys(const fgb_sort_options* opt, const char* header_text, size_t header_len,
                               const uint8_t* records, const uint64_t* rec_off, uint64_t n_records, uint64_t* keys,
                               uint64_t* bad_record);
-/* `fgumi sort --verify` (commands/sort.rs:376-408, 700-720): the records whose key is less than the previous record's
- * (template-coordinate: core_cmp, the first four words, inline_buffer.rs:604-618), and the index of the first of
- * them (UINT64_MAX when there is none). */
+/* The queryname key words the device's key kernel writes for one record (`len` bytes, no block_size prefix) when it
+ * is alone in its run: *n_words = W + 1, W name words (W = ceil(bound / 8), the bound on E from l_read_name:
+ * l_read_name - 1 bytes, natural 2 (l_read_name - 1) + 1, so at most 64) and the last word.  Within a run every record
+ * gets the run's largest W; the extra name words are 0.  A record shorter than 32 bytes gives FGB_ERR_LAYOUT; a cap
+ * below *n_words (which is still set), no words or an order other than the queryname ones give FGB_ERR_INVALID_ARG. */
+fgb_status fgb_host_sort_name_key(const fgb_sort_options* opt, const uint8_t* record, uint64_t len, uint64_t* words,
+                                  uint32_t cap, uint32_t* n_words);
+/* `fgumi sort --verify` (commands/sort.rs:376-408, 692-720): the records whose key is less than the previous record's
+ * (template-coordinate: core_cmp, the first four words, inline_buffer.rs:604-618; queryname: the name comparator,
+ * then the flag order), and the index of the first of them (UINT64_MAX when there is none). */
 fgb_status fgb_host_sort_verify(const fgb_sort_options* opt, const char* header_text, size_t header_len,
                                 const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
                                 uint64_t* violations, uint64_t* first_violation, uint64_t* bad_record);

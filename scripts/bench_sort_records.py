@@ -9,7 +9,11 @@ reaches tens of millions of records, the size at which users sort.  Rows, one JS
     share of the H100 SXM data-sheet 3.35 TB/s (the gather time includes the scan of the output offsets);
   - the same input forced into --runs runs (device_bytes set from the input size), with the host merge's time;
   - sort_file on a BAM of --file-records records: read / inflate / split (read_bam), device (the sort call) and
-    compress (BGZF level 1), as wall seconds.
+    compress (BGZF level 1), as wall seconds;
+  - queryname order, lexicographic and natural, in one run and forced into --runs runs, on a second input: the same
+    number of records with Illumina-style names A00123:8:HJKLMDSXY:<lane>:<tile>:<x>:<y> in coordinate order, so that
+    the names arrive shuffled, with the key words per record and the number of them that vary (from the key words of
+    a 100 000-record sample; the device skips the others).  --queryname-only runs these rows alone.
 The card's name, power limit and max SM clock are read in the same run.
 """
 import argparse
@@ -108,6 +112,61 @@ def make_records(n_templates: int, cb: bool, mi: bool, seed: int = 1):
     return rec.reshape(-1), off
 
 
+def make_named_records(n: int, seed: int = 3):
+    """(bodies, rec_off) of n records of 2 x 75 bp templates with Illumina-style names (lane 1-4, tile 1101-2678, x
+    and y five digits; both mates share the name), R1 and R2 flags and 1 % secondary records, in coordinate order."""
+    rng = np.random.default_rng(seed)
+    L = 75
+    prefix = b"A00123:8:HJKLMDSXY:"
+    name_len = len(prefix) + 1 + 1 + 4 + 1 + 5 + 1 + 5 + 1   # fixed-width fields + NUL
+    size = 32 + name_len + 4 + (L + 1) // 2 + L
+    t = np.arange(n) // 2                                     # template of each record
+    n_t = int(t[-1]) + 1
+    fields = [rng.integers(1, 5, n_t), rng.integers(1101, 2679, n_t), rng.integers(10000, 32001, n_t),
+              rng.integers(10000, 40001, n_t)]
+    tid = rng.integers(0, 24, n).astype(np.int32)
+    pos = rng.integers(0, 249_000_000, n).astype(np.int32)
+    order = np.lexsort((pos, tid))                            # coordinate order: mates apart, names shuffled
+    tid, pos, t = tid[order], pos[order], t[order]
+    mate = order % 2
+    flag = (0x1 | np.where(mate == 0, 0x40, 0x80) | np.where(rng.random(n) < 0.01, 0x100, 0)).astype(np.uint16)
+    rec = np.zeros((n, size), np.uint8)
+    fixed = np.zeros(n, dtype=[("tid", "<i4"), ("pos", "<i4"), ("lrn", "u1"), ("mapq", "u1"), ("bin", "<u2"),
+                               ("ncig", "<u2"), ("flag", "<u2"), ("lseq", "<u4"), ("mtid", "<i4"), ("mpos", "<i4"),
+                               ("tlen", "<i4")])
+    fixed["tid"], fixed["pos"], fixed["lrn"], fixed["mapq"], fixed["bin"] = tid, pos, name_len, 60, 4680
+    fixed["ncig"], fixed["flag"], fixed["lseq"], fixed["mtid"], fixed["mpos"] = 1, flag, L, -1, -1
+    rec[:, 0:32] = fixed.view(np.uint8).reshape(n, 32)
+    at = 32
+    rec[:, at:at + len(prefix)] = np.frombuffer(prefix, np.uint8)
+    at += len(prefix)
+    for k, width in enumerate((1, 4, 5, 5)):
+        v = fields[k][t]
+        rec[:, at:at + width] = (48 + (v[:, None] // (10 ** np.arange(width - 1, -1, -1))) % 10).astype(np.uint8)
+        at += width
+        if k < 3:
+            rec[:, at] = ord(":")
+            at += 1
+    at += 1                                                   # the NUL
+    rec[:, at:at + 4] = np.frombuffer(struct.pack("<I", (L << 4) | 0), np.uint8)
+    pool = rng.integers(0, 256, size=(4096, size - at - 4), dtype=np.uint8)
+    rec[:, at + 4:] = pool[np.arange(n) % 4096]
+    off = np.arange(n + 1, dtype=np.uint64) * np.uint64(size)
+    return rec.reshape(-1), off
+
+
+def key_word_counts(sort, bodies, off, order, sample: int = 100_000):
+    """(key words per record, key words that vary) over a random sample of the records."""
+    n = len(off) - 1
+    idx = np.random.default_rng(0).choice(n, min(n, sample), replace=False)
+    keys = np.array([sort.name_key(bodies[int(off[i]):int(off[i + 1])].tobytes(), order) for i in idx], np.uint64)
+    rec0 = bodies[int(off[0]):int(off[1])]
+    lrn = int(rec0[8]) - 1
+    words = (lrn * (2 if order == "queryname::natural" else 1) + (1 if order == "queryname::natural" else 0) + 7) // 8
+    varying = int(np.count_nonzero(np.bitwise_and.reduce(keys, 0) != np.bitwise_or.reduce(keys, 0)))
+    return words + 1, varying
+
+
 def timed_sort(sort, order, cb, bodies, off, repeats, device_bytes=0):
     s = sort.RecordSorter(0, order, b"CB" if cb else None, device_bytes=device_bytes)
     s.sort(HEADER, bodies, off)                      # warm-up: module load, CUB's kernels, host pages
@@ -131,11 +190,32 @@ def main():
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--cb", action="store_true", help="a 16-base CB on every record")
     ap.add_argument("--mi", action="store_true", help="an MI on every record")
+    ap.add_argument("--queryname-only", action="store_true", help="only the queryname rows")
     a = ap.parse_args()
     import __graft_entry__ as g
     g.build()
     from fgumi_b200 import bamio, lib, sort
     info = card()
+    if not a.queryname_only:
+        coordinate_rows(a, bamio, lib, sort, info)
+    queryname_rows(a, sort, info)
+
+
+def queryname_rows(a, sort, info):
+    t0 = time.perf_counter()
+    bodies, off = make_named_records(a.records)
+    n = len(off) - 1
+    common = dict(records=n, input_bytes=int(off[-1]), generate_s=time.perf_counter() - t0, card=info)
+    for order in ("queryname", "queryname::natural"):
+        words, varying = key_word_counts(sort, bodies, off, order)
+        budget = (int(off[-1]) * 2 + n * (68 + 8 * words + 4)) // a.runs + 1
+        for case, repeats, device_bytes in (("one_run", a.repeats, 0), ("forced_runs", 1, budget)):
+            wall, tm, _ = timed_sort(sort, order, False, bodies, off, repeats, device_bytes)
+            print(json.dumps(dict(case=case, order=order, device_bytes=device_bytes, wall_s=wall, records_per_s=n / wall,
+                                  key_words=words, varying_key_words_in_sample=varying, **tm, **common)), flush=True)
+
+
+def coordinate_rows(a, bamio, lib, sort, info):
     t0 = time.perf_counter()
     bodies, off = make_records(a.records // 2, a.cb, a.mi)
     n = len(off) - 1
