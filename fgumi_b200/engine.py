@@ -88,6 +88,8 @@ def pack_source_reads(units: Sequence[Sequence[Tuple[bytes, bytes]]], min_reads:
             if len(b) != len(q):
                 raise ValueError("bases/quals length mismatch")
             ln = len(b)
+            if ln > _l.FGB_MAX_READ_LEN:     # the descriptor's low 16 bits; a longer row would spill into its offset
+                raise ValueError(f"a row of {ln} bases is longer than FGB_MAX_READ_LEN ({_l.FGB_MAX_READ_LEN})")
             lens.append(ln)
             reads[r] = (off << 16) | ln
             pad = _round_up(ln, _l.FGB_READ_ALIGN) - ln

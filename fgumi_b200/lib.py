@@ -24,6 +24,7 @@ FGB_ERR_NOT_ENCODABLE = 9
 
 FGB_READ_ALIGN = 8
 FGB_OUT_ALIGN = 8
+FGB_MAX_READ_LEN = 65535     # a row descriptor holds 16 bits of length
 FGB_NCOUNTERS = 12
 COUNTER_NAMES = (
     "units", "positions", "exact_positions", "nocall_positions", "input_reads",
