@@ -250,6 +250,43 @@ def group_file(in_path: str, out_path: str, grouper, n_threads: int = 4, level: 
     return tm
 
 
+def dedup_records(text: bytes, bodies: np.ndarray, rec_off: np.ndarray, deduper, cell_tag: bytes = b"CB") -> bytes:
+    """`fgumi dedup` on a template-coordinate-sorted record stream in memory: position grouping that keeps secondary
+    and supplementary records, then the deduper; the MI-tagged stream with duplicates flagged 0x400 (or removed)."""
+    from .dedup import group_by_position
+    check_group_sort_order(text, False)   # is_template_coordinate_sorted (dedup.rs:971-978)
+    _, groups = group_by_position(bodies, rec_off, text, cell_tag)
+    deduper.add_groups(bodies, rec_off, groups)
+    return deduper.flush()
+
+
+def dedup_file(in_path: str, out_path: str, deduper, n_threads: int = 4, level: int = 1,
+               cell_tag: bytes = b"CB") -> Dict[str, float]:
+    """`fgumi dedup -i sorted.bam -o deduped.bam` with an existing dedup.Deduper (its options decide the rest).  Like
+    the reference (dedup.rs:1167-1179) it raises ValueError after writing the output when secondary or supplementary
+    records of this input lack the `tc` tag; the deduper may be reused across inputs."""
+    lib = _l.load()
+    text, bodies, rec_off, tm = read_bam(in_path, n_threads)
+    missing_before = deduper.stats()["missing_tc_tag"]   # a deduper may have run on other input before
+    t0 = time.perf_counter()
+    stream = dedup_records(text, bodies, rec_off, deduper, cell_tag)
+    t1 = time.perf_counter()
+    payload = mapped_bam_header(group_header(text, "fgumi_b200 dedup")) + stream
+    cap = lib.fgb_bgzf_bound(len(payload))
+    comp = np.empty(cap, dtype=np.uint8)
+    cn = C.c_size_t()
+    st = lib.fgb_bgzf_compress(payload, len(payload), level, n_threads, 1, comp.ctypes.data, cap, C.addressof(cn))
+    if st != 0:
+        raise _l.FgbError(st, "fgb_bgzf_compress")
+    comp[:cn.value].tofile(out_path)
+    tm.update({"dedup_s": t1 - t0, "input_records": float(len(rec_off) - 1), "output_bytes": float(len(payload))})
+    missing = deduper.stats()["missing_tc_tag"] - missing_before
+    if missing:
+        raise ValueError(f"{missing} secondary/supplementary reads are missing the `tc` tag, which correct UMI-aware "
+                         "deduplication of secondary and supplementary alignments needs (`fgumi zipper` adds it)")
+    return tm
+
+
 def split_stream(stream: bytes) -> Tuple[np.ndarray, np.ndarray]:
     """[u32 block_size][record]... -> (record bodies back to back, rec_off) through fgb_bam_split_records."""
     lib = _l.load()

@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libfgumi_b200.so")
 SOURCES = ["capi.cu", "host_tables.cpp", "host/caller_host.cpp", "host/bgzf.cpp", "host/umi_host.cpp",
-           "host/group_host.cpp", "host/sort_host.cpp"]
+           "host/group_host.cpp", "host/sort_host.cpp", "host/dedup_host.cpp"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-maxrregcount=112",      # upper bound only; vote_kernel must land at <= 96 (see _check_vote_kernel)
@@ -73,6 +73,19 @@ def _check_sort_kernels(ptxas_log: str) -> None:
         raise RuntimeError(f"fgumi_b200 build: ptxas reported {found} sort key / gather kernels, expected 4")
 
 
+def _check_score_kernel(ptxas_log: str) -> None:
+    """The template-score kernel keeps one accumulator and a uint4 per lane: a stack frame or a spill means a source
+    change pushed its state into local memory, and fails the build."""
+    import re
+    m = re.search(r"Function properties for (\S*dedup_score_kernel\S*)\n\s*(\d+) bytes stack frame, (\d+) bytes spill "
+                  r"stores", ptxas_log)
+    if not m:
+        raise RuntimeError("fgumi_b200 build: ptxas reported no dedup_score_kernel")
+    if int(m.group(2)) or int(m.group(3)):
+        raise RuntimeError(f"fgumi_b200 build: {m.group(1)} has a {m.group(2)}-byte stack frame and spills "
+                           f"{m.group(3)} bytes (expected none)")
+
+
 def build(force: bool = False, verbose: bool = False) -> str:
     deps = [os.path.join(dp, f) for dp, _, fs in os.walk(CSRC) for f in fs]
     deps.append(os.path.join(HERE, "..", "include", "fgumi_b200.h"))
@@ -88,6 +101,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     _check_vote_kernel(r.stdout + r.stderr)
     _check_umi_kernels(r.stdout + r.stderr)
     _check_sort_kernels(r.stdout + r.stderr)
+    _check_score_kernel(r.stdout + r.stderr)
     return OUT
 
 

@@ -16,6 +16,7 @@
 #include "../../include/fgumi_b200.h"
 #include "assemble_kernel.cuh"
 #include "combine_kernels.cuh"
+#include "dedup_kernels.cuh"
 #include "fgb_config.h"
 #include "filter_kernel.cuh"
 #include "inflate_kernel.cuh"
@@ -24,6 +25,7 @@
 #include "sort_kernels.cuh"
 #include "umi_kernels.cuh"
 #include "unpack_kernels.cuh"
+#include "host/dedup_device.h"
 #include "host/sort_device.h"
 #include "host/umi_host.h"
 #include <cub/device/device_radix_sort.cuh>
@@ -126,6 +128,15 @@ struct fgb_handle {
     double timing[4] = {0, 0, 0, 0};                 // fgb_umi_last_timing
   } umi;
   double sort_timing[6] = {0, 0, 0, 0, 0, 0};        // fgb_sort_last_timing
+  struct ScoreBufs {                                 // template scores (dedup_kernels.cuh): own stream, so that they run
+    cudaStream_t stream = nullptr;                   // beside fgb_umi_assign; two page-locked chunks alternate
+    uint8_t* h_rec[2] = {nullptr, nullptr}; uint64_t* h_off[2] = {nullptr, nullptr};
+    uint8_t* d_rec[2] = {nullptr, nullptr}; uint64_t* d_off[2] = {nullptr, nullptr};
+    uint64_t cap_rec = 0, cap_off = 0;               // bytes / entries of each of the four chunk buffers
+    uint32_t* d_scores = nullptr; uint32_t* h_scores = nullptr; uint64_t cap_scores = 0;
+    cudaEvent_t staged[2] = {nullptr, nullptr};      // the chunk's upload has left its page-locked buffers
+    std::vector<cudaEvent_t> ev;                     // kernel start / stop per chunk
+  } score;
 };
 
 namespace {
@@ -378,6 +389,16 @@ void fgb_destroy(fgb_handle* h) {
     cudaFreeHost(u.h_keys); cudaFreeHost(u.h_blob); cudaFreeHost(u.h_work); cudaFreeHost(u.h_sbits);
     cudaFreeHost(u.h_sidx); cudaFreeHost(u.h_off); cudaFreeHost(u.h_edges);
     for (cudaEvent_t ev : {u.ev0, u.ev1, u.ev2, u.ev3}) if (ev) cudaEventDestroy(ev);
+  }
+  {
+    auto& c = h->score;
+    if (c.stream) { cudaStreamSynchronize(c.stream); cudaStreamDestroy(c.stream); }
+    for (int b = 0; b < 2; ++b) {
+      cudaFreeHost(c.h_rec[b]); cudaFreeHost(c.h_off[b]); cudaFree(c.d_rec[b]); cudaFree(c.d_off[b]);
+      if (c.staged[b]) cudaEventDestroy(c.staged[b]);
+    }
+    cudaFree(c.d_scores); cudaFreeHost(c.h_scores);
+    for (cudaEvent_t ev : c.ev) cudaEventDestroy(ev);
   }
   if (h->ev_recstr) cudaEventDestroy(h->ev_recstr);
   delete h;
@@ -1767,3 +1788,155 @@ cudaError_t gather(const uint8_t* rec, const uint64_t* off, uint64_t base, const
 
 }  // namespace sortdev
 }  // namespace fgb
+
+// ---- template scores (dedup_kernels.cuh; the deduper is host/dedup_host.cpp) ----------------------------------------
+namespace fgb {
+namespace dedupdev {
+
+namespace {
+
+constexpr uint64_t kScoreStageBytes = 16ull << 20;   // one page-locked chunk of records (two alternate)
+
+// The chunk buffers for `bytes` of records and `entries` offsets, grown (never shrunk) without touching last_error:
+// a failure here is reported through the caller's string, since fgb_umi_assign may run on the handle meanwhile.
+cudaError_t score_buffers(fgb_handle* h, uint64_t bytes, uint64_t entries, uint64_t n) {
+  auto& c = h->score;
+  cudaError_t e;
+  if (!c.stream && (e = cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking)) != cudaSuccess) return e;
+  for (int b = 0; b < 2; ++b)
+    if (!c.staged[b] && (e = cudaEventCreateWithFlags(&c.staged[b], cudaEventDisableTiming)) != cudaSuccess) return e;
+  if (bytes > c.cap_rec) {
+    const uint64_t cap = bytes + bytes / 8 + 64;
+    for (int b = 0; b < 2; ++b) {
+      cudaFreeHost(c.h_rec[b]); cudaFree(c.d_rec[b]);
+      c.h_rec[b] = nullptr; c.d_rec[b] = nullptr;
+    }
+    c.cap_rec = 0;
+    for (int b = 0; b < 2; ++b)
+      if ((e = cudaHostAlloc(reinterpret_cast<void**>(&c.h_rec[b]), cap, cudaHostAllocDefault)) != cudaSuccess ||
+          (e = cudaMalloc(reinterpret_cast<void**>(&c.d_rec[b]), cap)) != cudaSuccess)
+        return e;
+    c.cap_rec = cap;
+  }
+  if (entries > c.cap_off) {
+    const uint64_t cap = entries + entries / 8 + 64;
+    for (int b = 0; b < 2; ++b) {
+      cudaFreeHost(c.h_off[b]); cudaFree(c.d_off[b]);
+      c.h_off[b] = nullptr; c.d_off[b] = nullptr;
+    }
+    c.cap_off = 0;
+    for (int b = 0; b < 2; ++b)
+      if ((e = cudaHostAlloc(reinterpret_cast<void**>(&c.h_off[b]), cap * 8, cudaHostAllocDefault)) != cudaSuccess ||
+          (e = cudaMalloc(reinterpret_cast<void**>(&c.d_off[b]), cap * 8)) != cudaSuccess)
+        return e;
+    c.cap_off = cap;
+  }
+  if (n > c.cap_scores) {
+    const uint64_t cap = n + n / 8 + 64;
+    cudaFree(c.d_scores); cudaFreeHost(c.h_scores);
+    c.d_scores = nullptr; c.h_scores = nullptr; c.cap_scores = 0;
+    if ((e = cudaMalloc(reinterpret_cast<void**>(&c.d_scores), cap * 4)) != cudaSuccess ||
+        (e = cudaHostAlloc(reinterpret_cast<void**>(&c.h_scores), cap * 4, cudaHostAllocDefault)) != cudaSuccess)
+      return e;
+    c.cap_scores = cap;
+  }
+  return cudaSuccess;
+}
+
+}  // namespace
+
+fgb_status quality_scores(fgb_handle* h, uint64_t n, const uint8_t* const* rec, const uint64_t* len, uint32_t n_threads,
+                          uint32_t* scores, float* kernel_ms, std::string* err) {
+  *kernel_ms = 0.f;
+  if (!n) return FGB_OK;
+  auto fail = [&](cudaError_t e, const char* what) {
+    *err = std::string("template scores: ") + what + ": " + cudaGetErrorString(e);
+    return e == cudaErrorMemoryAllocation ? FGB_ERR_NOMEM : FGB_ERR_CUDA;
+  };
+  cudaError_t e = cudaSetDevice(h->device);
+  if (e != cudaSuccess) return fail(e, "cudaSetDevice");
+  // chunks: as many consecutive records as fit one staging buffer (at least one)
+  std::vector<uint64_t> chunk{0};
+  uint64_t max_bytes = 0, max_n = 0;
+  for (uint64_t i = 0; i < n;) {
+    uint64_t bytes = len[i], j = i + 1;
+    while (j < n && bytes + len[j] <= kScoreStageBytes) bytes += len[j++];
+    max_bytes = std::max(max_bytes, bytes);
+    max_n = std::max(max_n, j - i);
+    chunk.push_back(j);
+    i = j;
+  }
+  const uint64_t n_chunks = chunk.size() - 1;
+  if ((e = score_buffers(h, max_bytes + 16, max_n + 1, n)) != cudaSuccess) { cudaGetLastError(); return fail(e, "buffers"); }
+  auto& c = h->score;
+  while (c.ev.size() < 2 * n_chunks) {
+    cudaEvent_t ev;
+    if ((e = cudaEventCreate(&ev)) != cudaSuccess) return fail(e, "cudaEventCreate");
+    c.ev.push_back(ev);
+  }
+  const unsigned max_grid = static_cast<unsigned>(std::max(h->sm_count, 1)) * 8;
+  for (uint64_t k = 0; k < n_chunks; ++k) {
+    const int b = static_cast<int>(k & 1);
+    const uint64_t i0 = chunk[k], cnt = chunk[k + 1] - i0;
+    if ((e = cudaEventSynchronize(c.staged[b])) != cudaSuccess) return fail(e, "cudaEventSynchronize");
+    uint64_t* off = c.h_off[b];
+    off[0] = 0;
+    for (uint64_t x = 0; x < cnt; ++x) off[x + 1] = off[x] + len[i0 + x];
+    const uint64_t t = std::min<uint64_t>(std::max<uint32_t>(n_threads, 1), std::max<uint64_t>(off[cnt] >> 22, 1));
+    fgb_umi::parallel_for(t, n_threads, [&](uint64_t w) {
+      for (uint64_t x = cnt * w / t, xe = cnt * (w + 1) / t; x < xe; ++x)
+        std::memcpy(c.h_rec[b] + off[x], rec[i0 + x], len[i0 + x]);
+    });
+    if ((e = cudaMemcpyAsync(c.d_rec[b], c.h_rec[b], off[cnt], cudaMemcpyHostToDevice, c.stream)) != cudaSuccess ||
+        (e = cudaMemcpyAsync(c.d_off[b], off, (cnt + 1) * 8, cudaMemcpyHostToDevice, c.stream)) != cudaSuccess ||
+        (e = cudaEventRecord(c.staged[b], c.stream)) != cudaSuccess)
+      return fail(e, "upload");
+    const unsigned grid = static_cast<unsigned>(std::min<uint64_t>((cnt + kScoreThreads / 32 - 1) / (kScoreThreads / 32), max_grid));
+    if ((e = cudaEventRecord(c.ev[2 * k], c.stream)) != cudaSuccess) return fail(e, "cudaEventRecord");
+    dedup_score_kernel<<<grid, kScoreThreads, 0, c.stream>>>(c.d_rec[b], c.d_off[b], static_cast<uint32_t>(cnt),
+                                                              c.d_scores + i0);
+    if ((e = cudaGetLastError()) != cudaSuccess) return fail(e, "dedup_score_kernel");
+    if ((e = cudaEventRecord(c.ev[2 * k + 1], c.stream)) != cudaSuccess) return fail(e, "cudaEventRecord");
+  }
+  if ((e = cudaMemcpyAsync(c.h_scores, c.d_scores, n * 4, cudaMemcpyDeviceToHost, c.stream)) != cudaSuccess ||
+      (e = cudaStreamSynchronize(c.stream)) != cudaSuccess)
+    return fail(e, "download");
+  std::memcpy(scores, c.h_scores, n * 4);
+  for (uint64_t k = 0; k < n_chunks; ++k) {
+    float ms = 0.f;
+    if ((e = cudaEventElapsedTime(&ms, c.ev[2 * k], c.ev[2 * k + 1])) != cudaSuccess) return fail(e, "cudaEventElapsedTime");
+    *kernel_ms += ms;
+  }
+  return FGB_OK;
+}
+
+}  // namespace dedupdev
+}  // namespace fgb
+
+extern "C" {
+
+fgb_status fgb_record_quality_scores(fgb_handle* h, const uint8_t* records, const uint64_t* rec_off,
+                                     uint64_t n_records, uint32_t* scores) {
+  if (!h || (n_records && (!records || !rec_off || !scores))) return FGB_ERR_INVALID_ARG;
+  if (h->submit_pending) { h->last_error = "fgb_record_quality_scores: a submit has not been waited on"; return FGB_ERR_BUSY; }
+  for (uint64_t i = 0; i < n_records; ++i)
+    if (rec_off[i + 1] < rec_off[i] || rec_off[i + 1] - rec_off[i] < 32) {
+      h->last_error = "fgb_record_quality_scores: record " + std::to_string(i) + " is shorter than 32 bytes";
+      return FGB_ERR_LAYOUT;
+    }
+  try {
+    std::vector<const uint8_t*> rp(n_records);
+    std::vector<uint64_t> rl(n_records);
+    for (uint64_t i = 0; i < n_records; ++i) { rp[i] = records + rec_off[i]; rl[i] = rec_off[i + 1] - rec_off[i]; }
+    float kernel_ms = 0.f;
+    std::string err;
+    const fgb_status st = fgb::dedupdev::quality_scores(h, n_records, rp.data(), rl.data(), 1, scores, &kernel_ms, &err);
+    if (st != FGB_OK) h->last_error = "fgb_record_quality_scores: " + err;
+    return st;
+  } catch (const std::bad_alloc&) {
+    h->last_error = "fgb_record_quality_scores: out of host memory";
+    return FGB_ERR_NOMEM;
+  }
+}
+
+}  // extern "C"

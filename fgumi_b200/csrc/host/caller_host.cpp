@@ -2712,6 +2712,7 @@ uint32_t fgb_struct_size(uint32_t id) {
     case 10: return sizeof(fgb_umi_options);
     case 11: return sizeof(fgb_group_options);
     case 12: return sizeof(fgb_sort_options);
+    case 13: return sizeof(fgb_dedup_options);
     default: return 0;
   }
 }

@@ -16,71 +16,14 @@
 
 #include "../../../include/fgumi_b200.h"
 #include "bam.h"
+#include "group_rules.h"
 #include "umi_host.h"
 
 namespace {
 
 using fgb::bam::View;
 namespace bam = fgb::bam;
-
-constexpr uint64_t kNone = UINT64_MAX;
-
-std::string_view read_name(const View& v) {
-  const uint32_t l = v.l_read_name();
-  return std::string_view(reinterpret_cast<const char*>(v.b + 32), l ? l - 1 : 0);
-}
-
-bool record_ok(const uint8_t* records, const uint64_t* rec_off, uint64_t i) {
-  if (rec_off[i + 1] < rec_off[i] || rec_off[i + 1] - rec_off[i] < 32) return false;
-  const View v(records + rec_off[i], rec_off[i + 1] - rec_off[i]);
-  return 32 + static_cast<size_t>(v.l_read_name()) <= v.n && v.cigar_in_bounds() && v.aux_off() <= v.n;
-}
-
-// tag_value_size (fields.rs:289-310); 0 = unknown type or truncated
-size_t tag_value_size(uint8_t t, const uint8_t* d, size_t n) {
-  switch (t) {
-    case 'A': case 'c': case 'C': return 1;
-    case 's': case 'S': return 2;
-    case 'i': case 'I': case 'f': return 4;
-    case 'Z': case 'H': {
-      const void* z = std::memchr(d, 0, n);
-      return z ? static_cast<const uint8_t*>(z) - d + 1 : 0;
-    }
-    case 'B': {
-      if (n < 5) return 0;
-      const uint8_t e = d[0];
-      const size_t es = (e == 'c' || e == 'C') ? 1 : (e == 's' || e == 'S') ? 2 : (e == 'i' || e == 'I' || e == 'f') ? 4 : 0;
-      return es ? 5 + static_cast<size_t>(bam::rd32(d + 1)) * es : 0;
-    }
-    default: return 0;
-  }
-}
-
-// unclipped_5prime_from_raw_bam (cigar.rs:201-228, 470-508): 1-based; 0 for an unmapped read, i32::MAX without CIGAR
-int32_t unclipped_5prime(const View& v) {
-  const uint16_t f = v.flags();
-  if (f & bam::kUnmapped) return 0;
-  const uint32_t n = v.n_cigar();
-  if (n == 0 || !v.cigar_in_bounds()) return INT32_MAX;
-  const int32_t pos = v.pos() + 1;
-  if (!(f & bam::kReverse)) {
-    int32_t clipped = 0;
-    for (uint32_t i = 0; i < n; ++i) {
-      const uint32_t op = v.cigar_op(i);
-      if ((op & 0xF) == 4 || (op & 0xF) == 5) clipped += static_cast<int32_t>(op >> 4);
-      else break;
-    }
-    return pos - clipped;
-  }
-  int32_t ref_len = 0, trailing = 0;
-  bool saw = false;
-  for (uint32_t i = 0; i < n; ++i) {
-    const uint32_t op = v.cigar_op(i);
-    if (bam::consumes_ref(op & 0xF)) { ref_len += static_cast<int32_t>(op >> 4); trailing = 0; saw = true; }
-    else if (((op & 0xF) == 4 || (op & 0xF) == 5) && saw) trailing += static_cast<int32_t>(op >> 4);
-  }
-  return pos + ref_len + trailing - 1;
-}
+using namespace fgb::grp;
 
 // ---- position grouping (unified_pipeline/bam.rs:415-499, base.rs:1375-1436, grouper.rs:406-588) ----------------
 struct PosKey {
@@ -121,10 +64,7 @@ struct Tpl {                    // one template's primary reads in its group's b
 struct GroupPrep {              // one position group after the host rules in front of the assignment
   std::vector<uint8_t> bytes;
   std::vector<Tpl> tpls;        // templates that passed the filter, in input order
-  std::vector<uint32_t> order;  // templates in call order (the calls concatenated)
-  std::vector<uint32_t> call_end;
-  std::string umis;             // per `order` entry: its UMI as umi_for_read made it
-  std::vector<uint64_t> umi_end;
+  Calls c;                      // the calls and their UMIs
   uint64_t filter[6] = {0, 0, 0, 0, 0, 0};
   bool dropped = false;         // the reference's assignment returns an error: nothing but the filter counts
 };
@@ -168,54 +108,13 @@ bool filter_template(const fgb_grouper& g, const View* r1, const View* r2, uint6
   for (const View* r : reads) {   // phase 2: one aux walk for MQ and the UMI (:157-221)
     if (!r) continue;
     const bool check_mq = !(r->flags() & bam::kMateUnmapped), check_umi = !g.opt.no_umi;
-    const uint8_t* a = r->b + r->aux_off();
-    const size_t an = r->n - r->aux_off();
-    bool have_mq = false, have_umi = false;
-    int64_t mq = 0;
-    const uint8_t* umi = nullptr;
-    size_t umi_len = 0;
-    size_t p = 0;
-    while (p + 3 <= an) {
-      const uint8_t t0 = a[p], t1 = a[p + 1], vt = a[p + 2];
-      if (check_umi && t0 == static_cast<uint8_t>(g.opt.umi_tag[0]) && t1 == static_cast<uint8_t>(g.opt.umi_tag[1]) && vt == 'Z') {
-        const void* z = std::memchr(a + p + 3, 0, an - (p + 3));
-        if (!z) break;
-        umi = a + p + 3;
-        umi_len = static_cast<const uint8_t*>(z) - umi;
-        have_umi = true;
-        p += 3 + umi_len + 1;
-        if (!check_mq || have_mq) break;
-        continue;
-      }
-      if (check_mq && t0 == 'M' && t1 == 'Q') {   // any integer type; a float or string MQ is None
-        const uint8_t* d = a + p + 3;
-        const size_t left = an - (p + 3);
-        have_mq = true;
-        switch (vt) {
-          case 'C': if (left >= 1) mq = d[0]; else have_mq = false; break;
-          case 'c': if (left >= 1) mq = static_cast<int8_t>(d[0]); else have_mq = false; break;
-          case 'S': if (left >= 2) mq = bam::rd16(d); else have_mq = false; break;
-          case 's': if (left >= 2) mq = static_cast<int16_t>(bam::rd16(d)); else have_mq = false; break;
-          case 'I': if (left >= 4) mq = bam::rd32(d); else have_mq = false; break;
-          case 'i': if (left >= 4) mq = bam::rdi32(d); else have_mq = false; break;
-          default: have_mq = false;
-        }
-      }
-      const size_t size = tag_value_size(vt, a + p + 3, an - (p + 3));
-      if (!size) break;
-      p += 3 + size;
-      if ((!check_umi || have_umi) && (!check_mq || have_mq)) break;
-    }
-    if (check_mq && have_mq && static_cast<uint8_t>(mq) < g.opt.min_map_q) { fc[F_POOR] += n; return false; }   // `as u8`
+    const MqUmi s = scan_mq_umi(*r, check_mq, check_umi, g.opt.umi_tag);
+    if (check_mq && s.have_mq && static_cast<uint8_t>(s.mq) < g.opt.min_map_q) { fc[F_POOR] += n; return false; }   // `as u8`
     if (g.opt.no_umi) continue;
-    if (!have_umi) { fc[F_POOR] += n; return false; }
-    size_t bases = 0;   // validate_umi (fgumi-umi lib.rs:323-333)
-    for (size_t i = 0; i < umi_len; ++i) {
-      const uint8_t c = umi[i];
-      if (c == 'N') { fc[F_NS] += n; return false; }
-      if (c == 'A' || c == 'C' || c == 'G' || c == 'T' || c == 'a' || c == 'c' || c == 'g' || c == 't') ++bases;
-    }
-    if (g.opt.umi.min_umi_length && bases < g.opt.umi.min_umi_length) { fc[F_SHORT] += n; return false; }
+    if (!s.have_umi) { fc[F_POOR] += n; return false; }
+    const int64_t bases = umi_bases(s.umi, s.umi_len);
+    if (bases < 0) { fc[F_NS] += n; return false; }
+    if (g.opt.umi.min_umi_length && static_cast<uint64_t>(bases) < g.opt.umi.min_umi_length) { fc[F_SHORT] += n; return false; }
   }
   fc[F_ACCEPTED] += n;
   return true;
@@ -264,104 +163,19 @@ std::string prepare_group(const fgb_grouper& g, const uint8_t* records, const ui
     i = j;
   }
   if (gp->tpls.empty()) return "";
-  // the orientation split (group.rs:373-422): sub-groups in (r1_positive, r2_positive) order, false first; paired
-  // strategies take the whole group as one call
-  const size_t nt = gp->tpls.size();
+  // the orientation split and each template's UMI; where the reference's assignment fails the group is dropped
+  // (group.rs:1512-1522)
   auto view_of = [&](uint64_t off, uint64_t len) { return View(gp->bytes.data() + off, len); };
-  if (g.umi.strategy != FGB_UMI_PAIRED) {
-    std::vector<uint8_t> ori(nt);
-    for (size_t t = 0; t < nt; ++t) {
-      const Tpl& x = gp->tpls[t];
-      const bool p1 = x.r1 == kNone || !(view_of(x.r1, x.r1_len).flags() & bam::kReverse);
-      const bool p2 = x.r2 == kNone || !(view_of(x.r2, x.r2_len).flags() & bam::kReverse);
-      ori[t] = static_cast<uint8_t>(p1 * 2 + p2);
-    }
-    for (uint8_t o = 0; o < 4; ++o) {
-      const size_t before = gp->order.size();
-      for (size_t t = 0; t < nt; ++t) if (ori[t] == o) gp->order.push_back(static_cast<uint32_t>(t));
-      if (gp->order.size() > before) gp->call_end.push_back(static_cast<uint32_t>(gp->order.size()));
-    }
-  } else {
-    gp->order.resize(nt);
-    std::iota(gp->order.begin(), gp->order.end(), 0u);
-    gp->call_end.push_back(static_cast<uint32_t>(nt));
+  std::vector<View> v1, v2;   // the copies' views (Tpl offsets), nullptr through the accessors when absent
+  for (const Tpl& x : gp->tpls) {
+    v1.push_back(view_of(x.r1 != kNone ? x.r1 : 0, x.r1_len));
+    v2.push_back(view_of(x.r2 != kNone ? x.r2 : 0, x.r2_len));
   }
-  // the UMI of each template (group.rs:440-477): R1's tag if R1 exists, else R2's; umi_for_read on it
-  gp->umi_end.reserve(nt);
-  std::vector<uint8_t> buf;
-  for (uint32_t t : gp->order) {
-    if (!g.opt.no_umi) {
-      const Tpl& x = gp->tpls[t];
-      const View v = x.r1 != kNone ? view_of(x.r1, x.r1_len) : view_of(x.r2, x.r2_len);
-      const uint8_t* val = nullptr;
-      size_t len = 0;
-      if (!bam::find_string_tag(v, g.opt.umi_tag, &val, &len)) {   // "Missing UMI tag": the group is dropped
-        gp->dropped = true;
-        return "";
-      }
-      if (!bam::valid_utf8(val, len)) { gp->dropped = true; return ""; }   // "Invalid UTF-8 in UMI"
-      bool r1_earlier = true;   // is_r1_genomically_earlier_raw (:268-279)
-      if (x.r1 != kNone && x.r2 != kNone) {
-        const View a = view_of(x.r1, x.r1_len), c = view_of(x.r2, x.r2_len);
-        r1_earlier = a.ref_id() != c.ref_id() ? a.ref_id() < c.ref_id() : unclipped_5prime(a) <= unclipped_5prime(c);
-      }
-      buf.resize(2 * len + 2 * g.umi.edits + 16);
-      size_t out_len = 0;
-      if (fgb_host_umi_for_read(&g.umi, val, len, r1_earlier, buf.data(), buf.size(), &out_len) != FGB_OK) {
-        gp->dropped = true;   // a paired UMI that is not two parts around one '-' (:311-317)
-        return "";
-      }
-      gp->umis.append(reinterpret_cast<const char*>(buf.data()), out_len);
-    }
-    gp->umi_end.push_back(gp->umis.size());   // no_umi: every UMI is "" (:446-448)
-  }
+  if (!split_and_umis(g.umi, g.opt.no_umi, g.opt.umi_tag, gp->tpls.size(),
+                      [&](size_t t) { return gp->tpls[t].r1 != kNone ? &v1[t] : nullptr; },
+                      [&](size_t t) { return gp->tpls[t].r2 != kNone ? &v2[t] : nullptr; }, &gp->c).empty())
+    gp->dropped = true;
   return "";
-}
-
-// update_string_tag (fgumi-raw-bam tags.rs:694-721) on a copy of `rec`, appended to `out`: the first entry of the
-// tag (of any type) has its value overwritten when the lengths agree (its type byte is kept), is replaced by a Z
-// entry when they differ; a record without the tag gets one appended.
-void emit_with_tag(const uint8_t* rec, size_t n, const char tag[2], std::string_view val, std::vector<uint8_t>* out) {
-  const View v(rec, n);
-  const size_t aux = v.aux_off();
-  size_t p = aux, start = kNone, end = 0;
-  while (aux < n && p + 3 <= n) {
-    const size_t size = tag_value_size(rec[p + 2], rec + p + 3, n - (p + 3));
-    if (rec[p] == static_cast<uint8_t>(tag[0]) && rec[p + 1] == static_cast<uint8_t>(tag[1])) {
-      if (size) { start = p; end = p + 3 + size; }
-      break;
-    }
-    if (!size) break;
-    p += 3 + size;
-  }
-  const uint32_t bs0 = 0;
-  const size_t at = out->size();
-  out->insert(out->end(), reinterpret_cast<const uint8_t*>(&bs0), reinterpret_cast<const uint8_t*>(&bs0) + 4);
-  const uint8_t* vb = reinterpret_cast<const uint8_t*>(val.data());
-  const uint8_t z[3] = {static_cast<uint8_t>(tag[0]), static_cast<uint8_t>(tag[1]), 'Z'};
-  if (start != kNone && end - start - 4 == val.size()) {
-    out->insert(out->end(), rec, rec + n);
-    std::memcpy(out->data() + at + 4 + start + 3, vb, val.size());
-  } else if (start != kNone) {
-    out->insert(out->end(), rec, rec + start);
-    out->insert(out->end(), z, z + 3);
-    out->insert(out->end(), vb, vb + val.size());
-    out->push_back(0);
-    out->insert(out->end(), rec + end, rec + n);
-  } else {
-    out->insert(out->end(), rec, rec + n);
-    out->insert(out->end(), z, z + 3);
-    out->insert(out->end(), vb, vb + val.size());
-    out->push_back(0);
-  }
-  const uint32_t bs = static_cast<uint32_t>(out->size() - at - 4);
-  std::memcpy(out->data() + at, &bs, 4);
-}
-
-void emit_plain(const uint8_t* rec, size_t n, std::vector<uint8_t>* out) {
-  const uint32_t bs = static_cast<uint32_t>(n);
-  out->insert(out->end(), reinterpret_cast<const uint8_t*>(&bs), reinterpret_cast<const uint8_t*>(&bs) + 4);
-  out->insert(out->end(), rec, rec + n);
 }
 
 void build_batch(fgb_grouper* g) {
@@ -372,10 +186,10 @@ void build_batch(fgb_grouper* g) {
     const GroupPrep& gp = g->queue[q];
     if (gp.dropped || gp.tpls.empty()) continue;
     const uint64_t base = g->b_umis.size();
-    g->b_umis.insert(g->b_umis.end(), gp.umis.begin(), gp.umis.end());
-    for (uint64_t e : gp.umi_end) g->b_umi_off.push_back(base + e);
+    g->b_umis.insert(g->b_umis.end(), gp.c.umis.begin(), gp.c.umis.end());
+    for (uint64_t e : gp.c.umi_end) g->b_umi_off.push_back(base + e);
     const uint64_t ub = g->b_call_off.back();
-    for (uint32_t e : gp.call_end) g->b_call_off.push_back(ub + e);
+    for (uint32_t e : gp.c.call_end) g->b_call_off.push_back(ub + e);
     g->b_group_off.push_back(g->b_call_off.size() - 1);
     g->b_group_of.push_back(q);
   }
@@ -395,12 +209,10 @@ void emit_group(const fgb_grouper& g, const GroupPrep& gp, const uint64_t* ids, 
   std::vector<uint64_t> tid(nt), vidx(nt);   // vidx: MoleculeId::to_vec_index + 1, 0 = None (sorts first)
   std::vector<uint8_t> tkind(nt);
   for (size_t u = 0; u < nt; ++u) {
-    const uint32_t t = gp.order[u];
+    const uint32_t t = gp.c.order[u];
     tkind[t] = kinds[u];
     tid[t] = ids[u];
-    vidx[t] = kinds[u] == FGB_MOL_NONE ? 0
-            : kinds[u] == FGB_MOL_SINGLE ? ids[u] + 1
-            : 2 * ids[u] + (kinds[u] == FGB_MOL_B) + 1;
+    vidx[t] = vec_index(kinds[u], ids[u]);
   }
   auto name = [&](size_t t) {
     return std::string_view(reinterpret_cast<const char*>(gp.bytes.data() + gp.tpls[t].name), gp.tpls[t].name_len);
@@ -420,11 +232,7 @@ void emit_group(const fgb_grouper& g, const GroupPrep& gp, const uint64_t* ids, 
   for (uint32_t t : sorted) {
     const Tpl& x = gp.tpls[t];
     const bool has = tkind[t] != FGB_MOL_NONE;
-    if (has) {
-      mi = std::to_string(tid[t] + base_mi);
-      if (tkind[t] == FGB_MOL_A) mi += "/A";
-      else if (tkind[t] == FGB_MOL_B) mi += "/B";
-    }
+    if (has) mi_string(tkind[t], tid[t], base_mi, &mi);
     for (auto [off, len] : {std::pair<uint64_t, uint64_t>{x.r1, x.r1_len}, {x.r2, x.r2_len}}) {
       if (off == kNone) continue;
       if (has) emit_with_tag(gp.bytes.data() + off, len, g.opt.assign_tag, mi, &go->bytes);
@@ -484,11 +292,10 @@ fgb_status guard(fgb_grouper* g, const char* where, F&& f) {
 
 }  // namespace
 
-extern "C" {
-
-fgb_status fgb_host_group_by_position(const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
-                                      const char* header_text, size_t header_len, const char* cell_tag,
-                                      uint8_t* keep, uint64_t* group_begin, uint64_t* n_groups, uint64_t* bad_record) {
+fgb_status fgb::grp::group_by_position(const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
+                                       const char* header_text, size_t header_len, const char* cell_tag,
+                                       bool include_secondary_supplementary, uint8_t* keep, uint64_t* group_begin,
+                                       uint64_t* n_groups, uint64_t* bad_record) {
   if (!keep || !group_begin || !n_groups || (n_records && (!records || !rec_off)) || (header_len && !header_text))
     return FGB_ERR_INVALID_ARG;
   if (bad_record) *bad_record = kNone;
@@ -498,12 +305,34 @@ fgb_status fgb_host_group_by_position(const uint8_t* records, const uint64_t* re
     PosKey cur{};
     bool have = false;
     uint64_t kept = 0, groups = 0, last = 0;
+    auto join = [&](uint64_t i, PosKey&& k) {
+      keep[i] = 1;
+      bool same = have && k == cur;
+      if (have && !same) {   // a new position continuing the previous record's QNAME stays (unmapped mates)
+        const View lv(records + rec_off[last], rec_off[last + 1] - rec_off[last]);
+        const View v(records + rec_off[i], rec_off[i + 1] - rec_off[i]);
+        same = read_name(lv) == read_name(v);
+      }
+      if (!same) { group_begin[groups++] = kept; cur = std::move(k); have = true; }
+      last = i;
+      ++kept;
+    };
     for (uint64_t i = 0; i < n_records; ++i) {
       if (!record_ok(records, rec_off, i)) { if (bad_record) *bad_record = i; return FGB_ERR_LAYOUT; }
       const View v(records + rec_off[i], rec_off[i + 1] - rec_off[i]);
       const uint16_t f = v.flags();
       keep[i] = 0;
-      if (f & (bam::kSecondary | bam::kSupplementary)) continue;   // grouper.rs:489-493
+      PosKey k{};
+      if (f & (bam::kSecondary | bam::kSupplementary)) {   // grouper.rs:489-493
+        if (!include_secondary_supplementary) continue;
+        // GroupKey::default() with only the name hash (bam.rs:431-435); MC is not validated (:452-475)
+        k.ref1 = INT32_MAX; k.pos1 = INT32_MAX; k.strand1 = UINT8_MAX;
+        k.ref2 = INT32_MAX; k.pos2 = INT32_MAX; k.strand2 = UINT8_MAX;
+        k.library = 0;
+        k.has_cell = false;
+        join(i, std::move(k));
+        continue;
+      }
       const uint8_t* val[3];
       size_t len[3];
       bam::find_string_tags(v, want, cell_tag ? 3 : 2, val, len);
@@ -513,7 +342,6 @@ fgb_status fgb_host_group_by_position(const uint8_t* records, const uint64_t* re
         if (bad_record) *bad_record = i;
         return FGB_ERR_INVALID_ARG;
       }
-      PosKey k{};
       k.library = 0;
       if (val[0]) {
         auto it = libs.find(std::string(reinterpret_cast<const char*>(val[0]), len[0]));
@@ -546,15 +374,7 @@ fgb_status fgb_host_group_by_position(const uint8_t* records, const uint64_t* re
           k.ref2 = own_ref; k.pos2 = own_pos; k.strand2 = strand;
         }
       }
-      keep[i] = 1;
-      bool same = have && k == cur;
-      if (have && !same) {   // a new position continuing the previous record's QNAME stays (unmapped mates)
-        const View lv(records + rec_off[last], rec_off[last + 1] - rec_off[last]);
-        same = read_name(lv) == read_name(v);
-      }
-      if (!same) { group_begin[groups++] = kept; cur = std::move(k); have = true; }
-      last = i;
-      ++kept;
+      join(i, std::move(k));
     }
     group_begin[groups] = kept;
     *n_groups = groups;
@@ -562,6 +382,23 @@ fgb_status fgb_host_group_by_position(const uint8_t* records, const uint64_t* re
     return FGB_ERR_NOMEM;
   }
   return FGB_OK;
+}
+
+extern "C" {
+
+fgb_status fgb_host_group_by_position(const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
+                                      const char* header_text, size_t header_len, const char* cell_tag,
+                                      uint8_t* keep, uint64_t* group_begin, uint64_t* n_groups, uint64_t* bad_record) {
+  return fgb::grp::group_by_position(records, rec_off, n_records, header_text, header_len, cell_tag, false, keep,
+                                     group_begin, n_groups, bad_record);
+}
+
+fgb_status fgb_host_dedup_group_by_position(const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
+                                            const char* header_text, size_t header_len, const char* cell_tag,
+                                            uint8_t* keep, uint64_t* group_begin, uint64_t* n_groups,
+                                            uint64_t* bad_record) {
+  return fgb::grp::group_by_position(records, rec_off, n_records, header_text, header_len, cell_tag, true, keep,
+                                     group_begin, n_groups, bad_record);
 }
 
 fgb_status fgb_grouper_create(int device, const fgb_group_options* opt, fgb_grouper** out) {

@@ -1,0 +1,265 @@
+// Record rules `fgumi group` and `fgumi dedup` share: record checks, the aux walk of their filters (MQ and the UMI in
+// one pass), the unclipped 5' end, the pair-orientation split with each template's UMI, and update_string_tag on
+// output.  Used by group_host.cpp and dedup_host.cpp; the citations are to fgumi 0.2.0 as there.
+#pragma once
+#include <cstdint>
+#include <cstring>
+#include <numeric>
+#include <string>
+#include <string_view>
+#include <vector>
+
+#include "../../../include/fgumi_b200.h"
+#include "bam.h"
+
+namespace fgb {
+namespace grp {
+
+using bam::View;
+
+constexpr uint64_t kNone = UINT64_MAX;
+
+inline std::string_view read_name(const View& v) {
+  const uint32_t l = v.l_read_name();
+  return std::string_view(reinterpret_cast<const char*>(v.b + 32), l ? l - 1 : 0);
+}
+
+inline bool record_ok(const uint8_t* records, const uint64_t* rec_off, uint64_t i) {
+  if (rec_off[i + 1] < rec_off[i] || rec_off[i + 1] - rec_off[i] < 32) return false;
+  const View v(records + rec_off[i], rec_off[i + 1] - rec_off[i]);
+  return 32 + static_cast<size_t>(v.l_read_name()) <= v.n && v.cigar_in_bounds() && v.aux_off() <= v.n;
+}
+
+// tag_value_size (fields.rs:289-310); 0 = unknown type or truncated
+inline size_t tag_value_size(uint8_t t, const uint8_t* d, size_t n) {
+  switch (t) {
+    case 'A': case 'c': case 'C': return 1;
+    case 's': case 'S': return 2;
+    case 'i': case 'I': case 'f': return 4;
+    case 'Z': case 'H': {
+      const void* z = std::memchr(d, 0, n);
+      return z ? static_cast<const uint8_t*>(z) - d + 1 : 0;
+    }
+    case 'B': {
+      if (n < 5) return 0;
+      const uint8_t e = d[0];
+      const size_t es = (e == 'c' || e == 'C') ? 1 : (e == 's' || e == 'S') ? 2 : (e == 'i' || e == 'I' || e == 'f') ? 4 : 0;
+      return es ? 5 + static_cast<size_t>(bam::rd32(d + 1)) * es : 0;
+    }
+    default: return 0;
+  }
+}
+
+// unclipped_5prime_from_raw_bam (cigar.rs:201-228, 470-508): 1-based; 0 for an unmapped read, i32::MAX without CIGAR
+inline int32_t unclipped_5prime(const View& v) {
+  const uint16_t f = v.flags();
+  if (f & bam::kUnmapped) return 0;
+  const uint32_t n = v.n_cigar();
+  if (n == 0 || !v.cigar_in_bounds()) return INT32_MAX;
+  const int32_t pos = v.pos() + 1;
+  if (!(f & bam::kReverse)) {
+    int32_t clipped = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+      const uint32_t op = v.cigar_op(i);
+      if ((op & 0xF) == 4 || (op & 0xF) == 5) clipped += static_cast<int32_t>(op >> 4);
+      else break;
+    }
+    return pos - clipped;
+  }
+  int32_t ref_len = 0, trailing = 0;
+  bool saw = false;
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t op = v.cigar_op(i);
+    if (bam::consumes_ref(op & 0xF)) { ref_len += static_cast<int32_t>(op >> 4); trailing = 0; saw = true; }
+    else if (((op & 0xF) == 4 || (op & 0xF) == 5) && saw) trailing += static_cast<int32_t>(op >> 4);
+  }
+  return pos + ref_len + trailing - 1;
+}
+
+// The filters' one aux walk for the mate's MQ and the UMI (group.rs:157-221, dedup.rs:299-361): the first UMI tag of
+// type Z, and MQ of any integer type widened to i64 (a float or string MQ, or a truncated one, is None).  The walk
+// stops once it has what it looks for, at an unknown type or at a truncated value.
+struct MqUmi {
+  bool have_mq = false, have_umi = false;
+  int64_t mq = 0;
+  const uint8_t* umi = nullptr;
+  size_t umi_len = 0;
+};
+
+inline MqUmi scan_mq_umi(const View& r, bool check_mq, bool check_umi, const char umi_tag[2]) {
+  MqUmi s;
+  const uint8_t* a = r.b + r.aux_off();
+  const size_t an = r.n - r.aux_off();
+  size_t p = 0;
+  while (p + 3 <= an) {
+    const uint8_t t0 = a[p], t1 = a[p + 1], vt = a[p + 2];
+    if (check_umi && t0 == static_cast<uint8_t>(umi_tag[0]) && t1 == static_cast<uint8_t>(umi_tag[1]) && vt == 'Z') {
+      const void* z = std::memchr(a + p + 3, 0, an - (p + 3));
+      if (!z) break;
+      s.umi = a + p + 3;
+      s.umi_len = static_cast<const uint8_t*>(z) - s.umi;
+      s.have_umi = true;
+      p += 3 + s.umi_len + 1;
+      if (!check_mq || s.have_mq) break;
+      continue;
+    }
+    if (check_mq && t0 == 'M' && t1 == 'Q') {
+      const uint8_t* d = a + p + 3;
+      const size_t left = an - (p + 3);
+      s.have_mq = true;
+      switch (vt) {
+        case 'C': if (left >= 1) s.mq = d[0]; else s.have_mq = false; break;
+        case 'c': if (left >= 1) s.mq = static_cast<int8_t>(d[0]); else s.have_mq = false; break;
+        case 'S': if (left >= 2) s.mq = bam::rd16(d); else s.have_mq = false; break;
+        case 's': if (left >= 2) s.mq = static_cast<int16_t>(bam::rd16(d)); else s.have_mq = false; break;
+        case 'I': if (left >= 4) s.mq = bam::rd32(d); else s.have_mq = false; break;
+        case 'i': if (left >= 4) s.mq = bam::rdi32(d); else s.have_mq = false; break;
+        default: s.have_mq = false;
+      }
+    }
+    const size_t size = tag_value_size(vt, a + p + 3, an - (p + 3));
+    if (!size) break;
+    p += 3 + size;
+    if ((!check_umi || s.have_umi) && (!check_mq || s.have_mq)) break;
+  }
+  return s;
+}
+
+// validate_umi (fgumi-umi lib.rs:323-333): -1 for an upper-case N, else the number of ACGT bases (either case)
+inline int64_t umi_bases(const uint8_t* umi, size_t len) {
+  int64_t bases = 0;
+  for (size_t i = 0; i < len; ++i) {
+    const uint8_t c = umi[i];
+    if (c == 'N') return -1;
+    if (c == 'A' || c == 'C' || c == 'G' || c == 'T' || c == 'a' || c == 'c' || c == 'g' || c == 't') ++bases;
+  }
+  return bases;
+}
+
+// The calls of one position group and the UMI of each template, as the assigner receives them.
+struct Calls {
+  std::vector<uint32_t> order;     // templates in call order (the calls concatenated)
+  std::vector<uint32_t> call_end;
+  std::string umis;                // per `order` entry: its UMI as umi_for_read made it
+  std::vector<uint64_t> umi_end;
+};
+
+// The orientation split (group.rs:373-422, dedup.rs:543-587): sub-groups in (r1_positive, r2_positive) order, false
+// first; paired strategies take the whole group as one call.  Then the UMI of each template (group.rs:440-477,
+// dedup.rs:498-529): R1's tag if R1 exists, else R2's, through umi_for_read; "" for every template with no_umi.
+// r1(t) / r2(t) give template t's primary reads (nullptr: absent).  Returns "" or why the reference's assignment
+// fails: group drops the position group, dedup fails the command.
+template <class R1, class R2>
+std::string split_and_umis(const fgb_umi_options& umi, bool no_umi, const char umi_tag[2], size_t nt, R1&& r1, R2&& r2,
+                           Calls* c) {
+  if (umi.strategy != FGB_UMI_PAIRED) {
+    std::vector<uint8_t> ori(nt);
+    for (size_t t = 0; t < nt; ++t) {
+      const View* a = r1(t);
+      const View* b = r2(t);
+      const bool p1 = !a || !(a->flags() & bam::kReverse);
+      const bool p2 = !b || !(b->flags() & bam::kReverse);
+      ori[t] = static_cast<uint8_t>(p1 * 2 + p2);
+    }
+    for (uint8_t o = 0; o < 4; ++o) {
+      const size_t before = c->order.size();
+      for (size_t t = 0; t < nt; ++t) if (ori[t] == o) c->order.push_back(static_cast<uint32_t>(t));
+      if (c->order.size() > before) c->call_end.push_back(static_cast<uint32_t>(c->order.size()));
+    }
+  } else {
+    c->order.resize(nt);
+    std::iota(c->order.begin(), c->order.end(), 0u);
+    c->call_end.push_back(static_cast<uint32_t>(nt));
+  }
+  c->umi_end.reserve(nt);
+  std::vector<uint8_t> buf;
+  for (uint32_t t : c->order) {
+    if (!no_umi) {
+      const View* a = r1(t);
+      const View* b = r2(t);
+      const View& v = a ? *a : *b;
+      const uint8_t* val = nullptr;
+      size_t len = 0;
+      if (!bam::find_string_tag(v, umi_tag, &val, &len)) return "No UMI tag found";
+      if (!bam::valid_utf8(val, len)) return "Invalid UTF-8 in UMI";
+      bool r1_earlier = true;   // is_r1_genomically_earlier_raw (group.rs:268-279, dedup.rs:460-469)
+      if (a && b)
+        r1_earlier = a->ref_id() != b->ref_id() ? a->ref_id() < b->ref_id() : unclipped_5prime(*a) <= unclipped_5prime(*b);
+      buf.resize(2 * len + 2 * umi.edits + 16);
+      size_t out_len = 0;
+      if (fgb_host_umi_for_read(&umi, val, len, r1_earlier, buf.data(), buf.size(), &out_len) != FGB_OK)
+        return "Paired strategy used but UMI did not contain 2 segments: " + std::string(reinterpret_cast<const char*>(val), len);
+      c->umis.append(reinterpret_cast<const char*>(buf.data()), out_len);
+    }
+    c->umi_end.push_back(c->umis.size());
+  }
+  return "";
+}
+
+// update_string_tag (fgumi-raw-bam tags.rs:694-721) on a copy of `rec`, appended to `out`: the first entry of the
+// tag (of any type) has its value overwritten when the lengths agree (its type byte is kept), is replaced by a Z
+// entry when they differ; a record without the tag gets one appended.
+inline void emit_with_tag(const uint8_t* rec, size_t n, const char tag[2], std::string_view val, std::vector<uint8_t>* out) {
+  const View v(rec, n);
+  const size_t aux = v.aux_off();
+  size_t p = aux, start = kNone, end = 0;
+  while (aux < n && p + 3 <= n) {
+    const size_t size = tag_value_size(rec[p + 2], rec + p + 3, n - (p + 3));
+    if (rec[p] == static_cast<uint8_t>(tag[0]) && rec[p + 1] == static_cast<uint8_t>(tag[1])) {
+      if (size) { start = p; end = p + 3 + size; }
+      break;
+    }
+    if (!size) break;
+    p += 3 + size;
+  }
+  const uint32_t bs0 = 0;
+  const size_t at = out->size();
+  out->insert(out->end(), reinterpret_cast<const uint8_t*>(&bs0), reinterpret_cast<const uint8_t*>(&bs0) + 4);
+  const uint8_t* vb = reinterpret_cast<const uint8_t*>(val.data());
+  const uint8_t z[3] = {static_cast<uint8_t>(tag[0]), static_cast<uint8_t>(tag[1]), 'Z'};
+  if (start != kNone && end - start - 4 == val.size()) {
+    out->insert(out->end(), rec, rec + n);
+    std::memcpy(out->data() + at + 4 + start + 3, vb, val.size());
+  } else if (start != kNone) {
+    out->insert(out->end(), rec, rec + start);
+    out->insert(out->end(), z, z + 3);
+    out->insert(out->end(), vb, vb + val.size());
+    out->push_back(0);
+    out->insert(out->end(), rec + end, rec + n);
+  } else {
+    out->insert(out->end(), rec, rec + n);
+    out->insert(out->end(), z, z + 3);
+    out->insert(out->end(), vb, vb + val.size());
+    out->push_back(0);
+  }
+  const uint32_t bs = static_cast<uint32_t>(out->size() - at - 4);
+  std::memcpy(out->data() + at, &bs, 4);
+}
+
+inline void emit_plain(const uint8_t* rec, size_t n, std::vector<uint8_t>* out) {
+  const uint32_t bs = static_cast<uint32_t>(n);
+  out->insert(out->end(), reinterpret_cast<const uint8_t*>(&bs), reinterpret_cast<const uint8_t*>(&bs) + 4);
+  out->insert(out->end(), rec, rec + n);
+}
+
+// The MI string of a molecule: its number plus the run's base, "/A" or "/B" for paired molecules
+inline void mi_string(uint8_t kind, uint64_t id, uint64_t base, std::string* mi) {
+  *mi = std::to_string(id + base);
+  if (kind == FGB_MOL_A) *mi += "/A";
+  else if (kind == FGB_MOL_B) *mi += "/B";
+}
+
+// MoleculeId::to_vec_index + 1 (lib.rs:112-119), 0 for None, so that None sorts first
+inline uint64_t vec_index(uint8_t kind, uint64_t id) {
+  return kind == FGB_MOL_NONE ? 0 : kind == FGB_MOL_SINGLE ? id + 1 : 2 * id + (kind == FGB_MOL_B) + 1;
+}
+
+// Position grouping of fgb_host_group_by_position and, with include_secondary_supplementary, of
+// fgb_host_dedup_group_by_position.  Defined in group_host.cpp.
+fgb_status group_by_position(const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
+                             const char* header_text, size_t header_len, const char* cell_tag,
+                             bool include_secondary_supplementary, uint8_t* keep, uint64_t* group_begin,
+                             uint64_t* n_groups, uint64_t* bad_record);
+
+}  // namespace grp
+}  // namespace fgb

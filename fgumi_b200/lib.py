@@ -211,6 +211,19 @@ GROUP_STAT_NAMES = ("total_records", "accepted_records", "discarded_non_pf", "di
 FGB_GROUP_HIST_FAMILY, FGB_GROUP_HIST_POSITION = 0, 1
 
 
+class FgbDedupOptions(C.Structure):
+    _fields_ = [("umi", FgbUmiOptions), ("min_map_q", C.c_uint8), ("include_non_pf", C.c_uint8),
+                ("no_umi", C.c_uint8), ("remove_duplicates", C.c_uint8), ("umi_tag", C.c_char * 2),
+                ("assign_tag", C.c_char * 2), ("first_mi", C.c_uint64)]
+
+
+FGB_DEDUP_NSTATS = 20
+DEDUP_STAT_NAMES = ("total_templates", "unique_templates", "duplicate_templates", "total_reads", "unique_reads",
+                    "duplicate_reads", "secondary_reads", "supplementary_reads", "missing_tc_tag", "total_records",
+                    "accepted_records", "discarded_non_pf", "discarded_poor_alignment", "discarded_ns_in_umi",
+                    "discarded_umi_too_short", "position_groups", "next_mi", "records_out")
+
+
 FGB_SORT_COORDINATE, FGB_SORT_TEMPLATE_COORDINATE, FGB_SORT_QUERYNAME, FGB_SORT_QUERYNAME_NATURAL = 0, 1, 2, 3
 
 
@@ -256,6 +269,9 @@ SYMBOLS = (
     "fgb_grouper_add_groups", "fgb_grouper_pending", "fgb_grouper_flush", "fgb_grouper_flush_with_ids",
     "fgb_grouper_stats", "fgb_grouper_histogram", "fgb_grouper_last_timing",
     "fgb_sort_records", "fgb_host_sort_keys", "fgb_host_sort_verify", "fgb_sort_last_timing", "fgb_host_sort_name_key",
+    "fgb_host_dedup_group_by_position", "fgb_deduper_create", "fgb_deduper_destroy", "fgb_deduper_last_error",
+    "fgb_deduper_add_groups", "fgb_deduper_pending", "fgb_deduper_flush", "fgb_deduper_flush_with_ids",
+    "fgb_deduper_stats", "fgb_deduper_histogram", "fgb_deduper_last_timing", "fgb_record_quality_scores",
 )
 
 _lib = None
@@ -461,6 +477,32 @@ def load() -> C.CDLL:
     lib.fgb_grouper_histogram.restype = C.c_int32
     lib.fgb_grouper_last_timing.argtypes = [vp, vp]
     lib.fgb_grouper_last_timing.restype = C.c_int32
+    lib.fgb_host_dedup_group_by_position.argtypes = [vp, vp, u64, C.c_char_p, C.c_size_t, C.c_char_p, vp, vp,
+                                                     C.POINTER(u64), C.POINTER(u64)]
+    lib.fgb_host_dedup_group_by_position.restype = C.c_int32
+    lib.fgb_deduper_create.argtypes = [C.c_int, C.POINTER(FgbDedupOptions), C.POINTER(vp)]
+    lib.fgb_deduper_create.restype = C.c_int32
+    lib.fgb_deduper_destroy.argtypes = [vp]
+    lib.fgb_deduper_destroy.restype = None
+    lib.fgb_deduper_last_error.argtypes = [vp, C.c_char_p, C.c_size_t]
+    lib.fgb_deduper_last_error.restype = C.c_size_t
+    lib.fgb_deduper_add_groups.argtypes = [vp, vp, vp, vp, u64]
+    lib.fgb_deduper_add_groups.restype = C.c_int32
+    lib.fgb_deduper_pending.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(u64), C.POINTER(vp),
+                                        C.POINTER(u64), C.POINTER(vp), C.POINTER(u64)]
+    lib.fgb_deduper_pending.restype = C.c_int32
+    lib.fgb_deduper_flush.argtypes = [vp, C.POINTER(vp), C.POINTER(u64), C.POINTER(u64)]
+    lib.fgb_deduper_flush.restype = C.c_int32
+    lib.fgb_deduper_flush_with_ids.argtypes = [vp, vp, vp, vp, vp, C.POINTER(vp), C.POINTER(u64), C.POINTER(u64)]
+    lib.fgb_deduper_flush_with_ids.restype = C.c_int32
+    lib.fgb_deduper_stats.argtypes = [vp, vp]
+    lib.fgb_deduper_stats.restype = C.c_int32
+    lib.fgb_deduper_histogram.argtypes = [vp, vp, vp, u64, C.POINTER(u64)]
+    lib.fgb_deduper_histogram.restype = C.c_int32
+    lib.fgb_deduper_last_timing.argtypes = [vp, vp]
+    lib.fgb_deduper_last_timing.restype = C.c_int32
+    lib.fgb_record_quality_scores.argtypes = [vp, vp, vp, u64, vp]
+    lib.fgb_record_quality_scores.restype = C.c_int32
     lib.fgb_sort_records.argtypes = [vp, C.POINTER(FgbSortOptions), C.c_char_p, C.c_size_t, vp, vp, u64, vp, u64,
                                      C.POINTER(u64), C.POINTER(u64)]
     lib.fgb_sort_records.restype = C.c_int32

@@ -979,6 +979,90 @@ fgb_status fgb_grouper_histogram(const fgb_grouper* g, int which, uint64_t* size
  * sort, tags and output stream on the host. */
 fgb_status fgb_grouper_last_timing(const fgb_grouper* g, double ms[5]);
 
+/* ---- `fgumi dedup` from raw records (src/lib/commands/dedup.rs; host code around fgb_umi_assign and the template
+ * score kernel, dedup_kernels.cuh)
+ * Position grouping for dedup (RecordPositionGrouper::with_secondary_supplementary, grouper.rs:437-444, 488-547):
+ * fgb_host_group_by_position with every record kept.  A secondary or supplementary record has the default key
+ * (unified_pipeline/bam.rs:431-435), so it joins the previous record's group when it continues that record's QNAME and
+ * otherwise opens a group of its own, which later such records join; MC is not checked on it.  Same arguments and
+ * errors as fgb_host_group_by_position. */
+fgb_status fgb_host_dedup_group_by_position(const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
+                                            const char* header_text, size_t header_len, const char* cell_tag,
+                                            uint8_t* keep, uint64_t* group_begin, uint64_t* n_groups,
+                                            uint64_t* bad_record);
+
+typedef struct fgb_dedup_options {
+  fgb_umi_options umi;      /* strategy / edits / min_umi_length / n_threads; rules must be FGB_UMI_RULES_MAPPED    */
+  uint8_t min_map_q;        /* 0 in the CLI; MQ tags are compared signed                                         */
+  uint8_t include_non_pf;   /* 0 */
+  uint8_t no_umi;           /* dedup by position only: identity, 0 edits, every UMI "" (dedup.rs:918-947)         */
+  uint8_t remove_duplicates;/* skip records flagged 0x400 in the output instead of emitting them                 */
+  char umi_tag[2];          /* "RX" */
+  char assign_tag[2];       /* "MI" */
+  uint64_t first_mi;        /* MI number of the first molecule                                                   */
+} fgb_dedup_options;
+
+enum {   /* fgb_deduper_stats: DedupMetrics (dedup.rs:71-92), FilterMetrics per TEMPLATE, and the deduper's counters */
+  FGB_DSTAT_TOTAL_TEMPLATES = 0, FGB_DSTAT_UNIQUE_TEMPLATES = 1, FGB_DSTAT_DUPLICATE_TEMPLATES = 2,
+  FGB_DSTAT_TOTAL_READS = 3, FGB_DSTAT_UNIQUE_READS = 4, FGB_DSTAT_DUPLICATE_READS = 5,
+  FGB_DSTAT_SECONDARY_READS = 6, FGB_DSTAT_SUPPLEMENTARY_READS = 7,
+  FGB_DSTAT_MISSING_TC_TAG = 8,    /* secondary / supplementary records of kept templates without a tc tag        */
+  FGB_DSTAT_FILTER_TOTAL = 9, FGB_DSTAT_FILTER_ACCEPTED = 10, FGB_DSTAT_FILTER_NON_PF = 11,
+  FGB_DSTAT_FILTER_POOR_ALIGNMENT = 12, FGB_DSTAT_FILTER_NS_IN_UMI = 13, FGB_DSTAT_FILTER_UMI_TOO_SHORT = 14,
+  FGB_DSTAT_POSITION_GROUPS = 15,  /* position groups added                                                      */
+  FGB_DSTAT_NEXT_MI = 16,          /* MI number of the next molecule                                             */
+  FGB_DSTAT_RECORDS_OUT = 17,
+  FGB_DEDUP_NSTATS = 20
+};
+
+/* The record-level deduper: process_position_group (dedup.rs:673-806) and its output (:1057-1138) per position group.
+ * add_groups (group g = records [group_rec[g], group_rec[g+1]), every record of the stream as
+ * fgb_host_dedup_group_by_position keeps it) runs on n_threads host threads: templates from consecutive records with
+ * one QNAME, records in Template::from_records order (R1, R2, R1 supplementaries reversed, R2 supplementaries reversed,
+ * R1 secondaries reversed, R2 secondaries reversed; template.rs:159-330), filter_template (dedup.rs:257-402; counts
+ * per template, both-unmapped always rejected, MQ compared signed), 0x400 cleared on every record of a passing
+ * template, the pair-orientation split (non-paired strategies), the UMI of R1 (else R2) through umi_for_read.  A
+ * template with two primary R1s (or R2s), a malformed record or an assignment error (a paired UMI without exactly one
+ * '-', a UMI that is not UTF-8; dedup.rs:717-719) fails the call and leaves nothing of it queued.
+ * flush scores the primary records of every queued template on the device (fgb_record_quality_scores, started before
+ * the assignment and waited for after it), sends every queued group through fgb_umi_assign, sorts each group's
+ * templates stably by (MoleculeId::to_vec_index, QNAME), None first, keeps in each family the first template of that
+ * order with the highest score (R1 score + R2 score) and flags every record of the others 0x400, and emits every record
+ * of every template in that order with the assign tag set (update_string_tag; a template without an ID unchanged),
+ * each with its block_size word; remove_duplicates skips records carrying 0x400.  Byte-identical for any n_threads.
+ * device == FGB_DEVICE_NONE: planning only -- flush fails with FGB_ERR_NO_DEVICE; pending exposes the UMI batch as it
+ * would go to fgb_umi_assign and flush_with_ids completes the flush from ids / kinds / group_mi_count and per-entry
+ * template scores (indexed like the pending batch) computed elsewhere.  Pointers stay valid as for fgb_grouper_*. */
+typedef struct fgb_deduper fgb_deduper;
+fgb_status fgb_deduper_create(int device, const fgb_dedup_options* opt, fgb_deduper** out);
+void fgb_deduper_destroy(fgb_deduper* d);
+size_t fgb_deduper_last_error(const fgb_deduper* d, char* buf, size_t buf_len);
+fgb_status fgb_deduper_add_groups(fgb_deduper* d, const uint8_t* records, const uint64_t* rec_off,
+                                  const uint64_t* group_rec, uint64_t n_groups);
+fgb_status fgb_deduper_pending(fgb_deduper* d, const uint8_t** umis, const uint64_t** umi_off, uint64_t* n_umis,
+                               const uint64_t** call_off, uint64_t* n_calls, const uint64_t** group_off,
+                               uint64_t* n_groups);
+fgb_status fgb_deduper_flush(fgb_deduper* d, const uint8_t** out, uint64_t* out_len, uint64_t* n_records);
+fgb_status fgb_deduper_flush_with_ids(fgb_deduper* d, const uint64_t* ids, const uint8_t* kinds,
+                                      const uint64_t* group_mi_count, const uint32_t* scores, const uint8_t** out,
+                                      uint64_t* out_len, uint64_t* n_records);
+fgb_status fgb_deduper_stats(const fgb_deduper* d, uint64_t stats[FGB_DEDUP_NSTATS]);
+/* Family sizes (templates per molecule, unassigned templates skipped) over every flush, ascending: *n entries,
+ * written only when cap >= *n (call with cap 0 to size). */
+fgb_status fgb_deduper_histogram(const fgb_deduper* d, uint64_t* sizes, uint64_t* counts, uint64_t cap, uint64_t* n);
+/* Where the last fgb_deduper_flush spent its time, in ms: [0..3] fgb_umi_last_timing of its assignment, [4] the score
+ * phase as the host saw it (staging, transfers, kernel, scores back), [5] the score kernel alone (CUDA events), [6]
+ * the selection, flags, tags and output stream on the host. */
+fgb_status fgb_deduper_last_timing(const fgb_deduper* d, double ms[7]);
+
+/* score_template's per-read term (dedup.rs:230-249) on the device: scores[i] = sum(min(q, 15)) over record i's quality
+ * bytes (record i = records[rec_off[i] .. rec_off[i+1]), no block_size prefix), read from qo = 32 + l_read_name +
+ * 4 n_cigar + (l_seq + 1) / 2 for min(l_seq, len - qo) bytes (0 when qo >= len): a record whose qualities are cut short
+ * by its end is clamped, and 0xFF qualities count 15.  Staged through page-locked chunks; synchronous.  A record
+ * shorter than 32 bytes (or a descending rec_off) gives FGB_ERR_LAYOUT, fgb_last_error naming its index. */
+fgb_status fgb_record_quality_scores(fgb_handle* h, const uint8_t* records, const uint64_t* rec_off,
+                                     uint64_t n_records, uint32_t* scores);
+
 /* ---- `fgumi sort` on raw records (src/lib/sort/, src/lib/commands/sort.rs): coordinate, template-coordinate and
  * queryname.  Keys (fgumi_b200/csrc/sort_keys.h, the same code on the host and the device):
  *   coordinate: one word, (tid << 34) | ((pos + 1) << 1) | reverse, all ones for tid < 0 (the unmapped flag is not
@@ -1045,7 +1129,8 @@ fgb_status fgb_sort_last_timing(const fgb_handle* h, double ms[6]);
 /* sizeof() of the ABI structs as this library was compiled, so a binding can check its own layout:
  * 0 fgb_caller_options, 1 fgb_filter_params, 2 fgb_submit_options, 3 fgb_raw_columns,
  * 4 fgb_raw_read, 5 fgb_batch, 6 fgb_codec_params, 7 fgb_params, 8 fgb_duplex_filter_params,
- * 9 fgb_record_columns, 10 fgb_umi_options, 11 fgb_group_options, 12 fgb_sort_options; 0 for an unknown id. */
+ * 9 fgb_record_columns, 10 fgb_umi_options, 11 fgb_group_options, 12 fgb_sort_options, 13 fgb_dedup_options; 0 for
+ * an unknown id. */
 uint32_t fgb_struct_size(uint32_t id);
 
 #ifdef __cplusplus
