@@ -329,3 +329,73 @@ def group_and_call(in_path: str, grouper, caller, n_threads: int = 4, cell_tag: 
     data, ln, cnt = C.c_void_p(), C.c_uint64(), C.c_uint64()
     caller._check(lib.fgb_caller_flush(caller._h, C.byref(data), C.byref(ln), C.byref(cnt)), "fgb_caller_flush")
     return ConsensusOutput(C.string_at(data.value, ln.value) if ln.value else b"", cnt.value)
+
+
+def qname_batches(bodies: np.ndarray, rec_off: np.ndarray, batch_records: int):
+    """[begin, end) record ranges of about batch_records records each, every cut at a QNAME change, so that each
+    range holds whole templates."""
+    n = len(rec_off) - 1
+    name = lambda i: bytes(bodies[int(rec_off[i]) + 32:int(rec_off[i]) + 32 + int(bodies[int(rec_off[i]) + 8])])
+    b = 0
+    while b < n:
+        e = min(n, b + max(1, batch_records))
+        while e < n and name(e) == name(e - 1):
+            e += 1
+        yield b, e
+        b = e
+
+
+def filter_file(in_path: str, out_path: str, record_filter, reference=None, rejects: str = None, stats: str = None,
+                n_threads: int = 4, level: int = 1, batch_records: int = 1_000_000) -> Dict[str, float]:
+    """`fgumi filter -i in.bam -o out.bam [--ref ref.fa] [--rejects rejects.bam] [--stats stats.txt]` with an existing
+    filter.RecordFilter (its options decide the rest; rejects need it made with track_rejects=True) and an optional
+    filter.Reference.  Both outputs get the input header with one @PG.  The input is read into memory whole; it is
+    filtered in batches of about batch_records records cut at QNAME changes, and each batch's output is compressed and
+    written before the next, so that the outputs are never held whole.  A failing batch raises with
+    record_filter.bad_record set to the index in the whole input."""
+    from .filter import filter_stats_text
+    lib = _l.load()
+    text, bodies, rec_off, tm = read_bam(in_path, n_threads)
+    header = mapped_bam_header(group_header(text, "fgumi_b200 filter"))
+    outs = [(open(path, "wb"), header) for path in (out_path, rejects) if path is not None]
+
+    def write(k, payload, eof):
+        cap = lib.fgb_bgzf_bound(len(payload))
+        comp = np.empty(max(cap, 1), dtype=np.uint8)
+        cn = C.c_size_t()
+        st = lib.fgb_bgzf_compress(payload, len(payload), level, n_threads, 1 if eof else 0, comp.ctypes.data, cap,
+                                   C.addressof(cn))
+        if st != 0:
+            raise _l.FgbError(st, "fgb_bgzf_compress")
+        outs[k][0].write(comp[:cn.value].tobytes())
+
+    counts = {"total": 0, "passed": 0, "failed": 0, "bases_masked": 0}
+    t_filter = out_bytes = 0.0
+    try:
+        for b, e in qname_batches(bodies, rec_off, batch_records):
+            t0 = time.perf_counter()
+            try:
+                kept, rej, c = record_filter.filter(text, bodies[int(rec_off[b]):int(rec_off[e])],
+                                                    rec_off[b:e + 1] - rec_off[b], reference)
+            except Exception:
+                if record_filter.bad_record is not None:
+                    record_filter.bad_record += b
+                raise
+            t_filter += time.perf_counter() - t0
+            for k in counts:
+                counts[k] += c[k]
+            out_bytes += len(kept)
+            for k, stream in enumerate((kept, rej)[:len(outs)]):
+                write(k, outs[k][1] + stream, False)
+                outs[k] = (outs[k][0], b"")   # the header goes with the first batch only
+        for k in range(len(outs)):
+            write(k, outs[k][1], True)          # the header of an empty input, and the EOF member
+    finally:
+        for f, _ in outs:
+            f.close()
+    if stats is not None:
+        with open(stats, "w") as f:
+            f.write(filter_stats_text(counts))
+    tm.update({"filter_s": t_filter, "input_records": float(len(rec_off) - 1), "output_bytes": float(out_bytes)})
+    tm.update({k: float(v) for k, v in counts.items()})
+    return tm

@@ -19,6 +19,7 @@
 #include "dedup_kernels.cuh"
 #include "fgb_config.h"
 #include "filter_kernel.cuh"
+#include "filter_records_kernels.cuh"
 #include "inflate_kernel.cuh"
 #include "host_tables.h"
 #include "planner.h"
@@ -26,6 +27,7 @@
 #include "umi_kernels.cuh"
 #include "unpack_kernels.cuh"
 #include "host/dedup_device.h"
+#include "host/filter_device.h"
 #include "host/sort_device.h"
 #include "host/umi_host.h"
 #include <cub/device/device_radix_sort.cuh>
@@ -128,6 +130,8 @@ struct fgb_handle {
     double timing[4] = {0, 0, 0, 0};                 // fgb_umi_last_timing
   } umi;
   double sort_timing[6] = {0, 0, 0, 0, 0, 0};        // fgb_sort_last_timing
+  double filter_timing[6] = {0, 0, 0, 0, 0, 0};      // fgb_filter_last_timing
+  std::vector<uint8_t> filter_kept, filter_rejects;  // fgb_filter_records' output streams
   struct ScoreBufs {                                 // template scores (dedup_kernels.cuh): own stream, so that they run
     cudaStream_t stream = nullptr;                   // beside fgb_umi_assign; two page-locked chunks alternate
     uint8_t* h_rec[2] = {nullptr, nullptr}; uint64_t* h_off[2] = {nullptr, nullptr};
@@ -1787,6 +1791,65 @@ cudaError_t gather(const uint8_t* rec, const uint64_t* off, uint64_t base, const
 }
 
 }  // namespace sortdev
+}  // namespace fgb
+
+// ---- record filter (filter_records_kernels.cuh; the driver is host/filter_host.cpp) ---------------------------------
+namespace fgb {
+namespace filterdev {
+
+HandleInfo info(fgb_handle* h) {
+  return HandleInfo{h->device,        h->sm_count,   h->slots[0].stream, h->submit_pending, &h->last_error,
+                    h->filter_timing, &h->filter_kept, &h->filter_rejects};
+}
+
+namespace {
+unsigned warp_grid(uint32_t n, int sm_count) {   // one warp per record, at most 16 CTAs per SM (grid-stride)
+  const uint64_t want = (static_cast<uint64_t>(n) * 32 + kFilterThreads - 1) / kFilterThreads;
+  return static_cast<unsigned>(std::max<uint64_t>(1, std::min<uint64_t>(want, static_cast<uint64_t>(sm_count) * 16)));
+}
+}  // namespace
+
+cudaError_t pass1(uint8_t* rec, const uint64_t* off, uint64_t base, uint32_t n, const FilterCfg& cfg,
+                  const int32_t* ctg_of_ref, const uint64_t* ctg_off, const uint64_t* ctg_len, const uint8_t* genome,
+                  uint64_t first, FRec* out, unsigned long long* err, unsigned long long* counters, int sm_count,
+                  cudaStream_t s) {
+  if (!n) return cudaSuccess;
+  filter_pass1_kernel<<<warp_grid(n, sm_count), kFilterThreads, 0, s>>>(rec, off, base, n, cfg, ctg_of_ref, ctg_off,
+                                                                       ctg_len, genome, first, out, err, counters);
+  return cudaGetLastError();
+}
+
+cudaError_t decide(FRec* fr, const uint32_t* order, const uint32_t* tpl, uint32_t n_tpl, bool by_template,
+                   unsigned long long* counters, cudaStream_t s) {
+  if (!n_tpl) return cudaSuccess;
+  filter_decide_kernel<<<(n_tpl + kFilterThreads - 1) / kFilterThreads, kFilterThreads, 0, s>>>(fr, order, tpl, n_tpl,
+                                                                                                 by_template, counters);
+  return cudaGetLastError();
+}
+
+cudaError_t offsets(void* temp, size_t* temp_bytes, const FRec* fr, const uint32_t* order, uint32_t n,
+                    bool track_rejects, uint64_t* ks, uint64_t* rs, uint64_t* koff, uint64_t* roff, cudaStream_t s) {
+  if (!temp) return cub::DeviceScan::ExclusiveSum(nullptr, *temp_bytes, ks, koff, static_cast<int>(n) + 1, s);
+  filter_sizes_kernel<<<(n + kFilterThreads) / kFilterThreads, kFilterThreads, 0, s>>>(fr, order, n, track_rejects, ks,
+                                                                                      rs);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  size_t tb = *temp_bytes;
+  if ((e = cub::DeviceScan::ExclusiveSum(temp, tb, ks, koff, static_cast<int>(n) + 1, s)) != cudaSuccess) return e;
+  tb = *temp_bytes;
+  return cub::DeviceScan::ExclusiveSum(temp, tb, rs, roff, static_cast<int>(n) + 1, s);
+}
+
+cudaError_t pass2(const uint8_t* rec, const uint64_t* off, uint64_t base, uint32_t n, const FRec* fr,
+                  const uint32_t* order, const uint64_t* koff, const uint64_t* roff, bool track_rejects,
+                  const uint8_t* genome, uint8_t* kept, uint8_t* rejects, int sm_count, cudaStream_t s) {
+  if (!n) return cudaSuccess;
+  filter_pass2_kernel<<<warp_grid(n, sm_count), kFilterThreads, 0, s>>>(rec, off, base, n, fr, order, koff, roff,
+                                                                       track_rejects, genome, kept, rejects);
+  return cudaGetLastError();
+}
+
+}  // namespace filterdev
 }  // namespace fgb
 
 // ---- template scores (dedup_kernels.cuh; the deduper is host/dedup_host.cpp) ----------------------------------------

@@ -2713,6 +2713,7 @@ uint32_t fgb_struct_size(uint32_t id) {
     case 11: return sizeof(fgb_group_options);
     case 12: return sizeof(fgb_sort_options);
     case 13: return sizeof(fgb_dedup_options);
+    case 14: return sizeof(fgb_record_filter_options);
     default: return 0;
   }
 }

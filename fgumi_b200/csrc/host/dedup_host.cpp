@@ -104,24 +104,17 @@ std::string prepare_group(const fgb_deduper& d, const uint8_t* records, const ui
   views.reserve(e - b);
   for (uint64_t i = b; i < e; ++i) views.emplace_back(records + rec_off[i], rec_off[i + 1] - rec_off[i]);
   const uint64_t n = e - b;
-  std::vector<uint64_t> r1_supp, r2_supp, r1_sec, r2_sec;
+  std::vector<uint64_t> lists[4], order;
   for (uint64_t i = 0; i < n;) {
     uint64_t j = i + 1;
     const std::string_view name = read_name(views[i]);
     while (j < n && read_name(views[j]) == name) ++j;
-    int64_t r1 = -1, r2 = -1;
-    r1_supp.clear(); r2_supp.clear(); r1_sec.clear(); r2_sec.clear();
-    for (uint64_t k = i; k < j; ++k) {
-      const uint16_t f = views[k].flags();
-      const bool is_r1 = !(f & bam::kPaired) || (f & bam::kFirst);
-      if (f & bam::kSecondary) { (is_r1 ? r1_sec : r2_sec).push_back(k); continue; }
-      if (f & bam::kSupplementary) { (is_r1 ? r1_supp : r2_supp).push_back(k); continue; }
-      int64_t& slot = is_r1 ? r1 : r2;
-      if (slot >= 0)
-        return std::string("Multiple non-secondary, non-supplemental ") + (is_r1 ? "R1" : "R2") + " records for read '" +
-               std::string(name) + "'";
-      slot = static_cast<int64_t>(k);
-    }
+    int64_t r1, r2;
+    uint64_t dup;
+    order.clear();
+    const std::string err = template_order(i, j, [&](uint64_t k) { return views[k].flags(); }, name, lists, &order,
+                                           &r1, &r2, &dup);
+    if (!err.empty()) return err;
     const View* v1 = r1 >= 0 ? &views[r1] : nullptr;
     const View* v2 = r2 >= 0 ? &views[r2] : nullptr;
     if (filter_template(d, v1, v2, gp->filter)) {
@@ -135,10 +128,11 @@ std::string prepare_group(const fgb_deduper& d, const uint8_t* records, const ui
         std::memcpy(gp->bytes.data() + at + 14, &f, 2);
         gp->recs.push_back(DRec{at, v.n});
       };
-      if (r1 >= 0) { t.r1 = static_cast<int64_t>(gp->recs.size()); copy(r1); }
-      if (r2 >= 0) { t.r2 = static_cast<int64_t>(gp->recs.size()); copy(r2); }
-      for (auto* list : {&r1_supp, &r2_supp, &r1_sec, &r2_sec})   // each reversed (fgbio's list prepend order)
-        for (auto it = list->rbegin(); it != list->rend(); ++it) copy(*it);
+      for (uint64_t k : order) {
+        if (static_cast<int64_t>(k) == r1) t.r1 = static_cast<int64_t>(gp->recs.size());
+        if (static_cast<int64_t>(k) == r2) t.r2 = static_cast<int64_t>(gp->recs.size());
+        copy(k);
+      }
       t.rec_end = gp->recs.size();
       t.name = gp->recs[t.rec_begin].off + 32;
       t.name_len = name.size();

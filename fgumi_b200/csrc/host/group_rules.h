@@ -136,6 +136,37 @@ inline int64_t umi_bases(const uint8_t* umi, size_t len) {
   return bases;
 }
 
+// build_templates_from_records + Template::from_records (grouper.rs:596-651, template.rs:159-330) for the records
+// k in [b, e) of one QNAME run, flags(k) giving each one's flags: appends them to `order` in template order -- R1, R2,
+// then the R1 and the R2 supplementary and the R1 and the R2 secondary records, each list reversed (fgbio's prepend
+// order; secondary wins over supplementary) -- and sets *r1 / *r2 to the primary reads (-1: absent).  The two-record
+// fast path's swap lands on the same order.  Returns "" or the reference's error for a second primary R1 or R2, with
+// *dup = that record.  `lists` is scratch.
+template <class Flags>
+std::string template_order(uint64_t b, uint64_t e, Flags&& flags, std::string_view name, std::vector<uint64_t> lists[4],
+                           std::vector<uint64_t>* order, int64_t* r1, int64_t* r2, uint64_t* dup) {
+  *r1 = -1;
+  *r2 = -1;
+  for (int l = 0; l < 4; ++l) lists[l].clear();   // r1 supp, r2 supp, r1 sec, r2 sec
+  for (uint64_t k = b; k < e; ++k) {
+    const uint16_t f = flags(k);
+    const bool is_r1 = !(f & bam::kPaired) || (f & bam::kFirst);
+    if (f & bam::kSecondary) { lists[is_r1 ? 2 : 3].push_back(k); continue; }
+    if (f & bam::kSupplementary) { lists[is_r1 ? 0 : 1].push_back(k); continue; }
+    int64_t& slot = is_r1 ? *r1 : *r2;
+    if (slot >= 0) {
+      *dup = k;
+      return std::string("Multiple non-secondary, non-supplemental ") + (is_r1 ? "R1" : "R2") + " records for read '" +
+             std::string(name) + "'";
+    }
+    slot = static_cast<int64_t>(k);
+  }
+  if (*r1 >= 0) order->push_back(static_cast<uint64_t>(*r1));
+  if (*r2 >= 0) order->push_back(static_cast<uint64_t>(*r2));
+  for (int l = 0; l < 4; ++l) order->insert(order->end(), lists[l].rbegin(), lists[l].rend());
+  return "";
+}
+
 // The calls of one position group and the UMI of each template, as the assigner receives them.
 struct Calls {
   std::vector<uint32_t> order;     // templates in call order (the calls concatenated)

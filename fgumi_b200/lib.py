@@ -232,6 +232,15 @@ class FgbSortOptions(C.Structure):
                 ("reserved", C.c_uint8 * 6), ("device_bytes", C.c_uint64)]
 
 
+class FgbRecordFilterOptions(C.Structure):
+    _fields_ = [("filter", FgbDuplexFilterParams), ("filter_by_template", C.c_uint8),
+                ("reverse_per_base_tags", C.c_uint8), ("track_rejects", C.c_uint8), ("reserved", C.c_uint8 * 1),
+                ("n_threads", C.c_uint32), ("device_bytes", C.c_uint64)]
+
+
+FILTER_STAT_NAMES = ("total", "passed", "failed", "bases_masked")
+
+
 class FgbUmiKey(C.Structure):
     _fields_ = [("bits", C.c_uint64), ("str_off", C.c_uint64), ("str_len", C.c_uint32), ("count", C.c_uint32),
                 ("first", C.c_uint32), ("dash", C.c_uint32), ("len", C.c_uint8), ("flags", C.c_uint8),
@@ -272,6 +281,8 @@ SYMBOLS = (
     "fgb_host_dedup_group_by_position", "fgb_deduper_create", "fgb_deduper_destroy", "fgb_deduper_last_error",
     "fgb_deduper_add_groups", "fgb_deduper_pending", "fgb_deduper_flush", "fgb_deduper_flush_with_ids",
     "fgb_deduper_stats", "fgb_deduper_histogram", "fgb_deduper_last_timing", "fgb_record_quality_scores",
+    "fgb_reference_create", "fgb_reference_destroy", "fgb_reference_contigs", "fgb_reference_contig",
+    "fgb_filter_records", "fgb_filter_last_timing",
 )
 
 _lib = None
@@ -516,6 +527,20 @@ def load() -> C.CDLL:
     lib.fgb_host_sort_name_key.restype = C.c_int32
     lib.fgb_sort_last_timing.argtypes = [vp, vp]
     lib.fgb_sort_last_timing.restype = C.c_int32
+    lib.fgb_reference_create.argtypes = [C.c_int, vp, C.c_size_t, C.POINTER(vp)]
+    lib.fgb_reference_create.restype = C.c_int32
+    lib.fgb_reference_destroy.argtypes = [vp]
+    lib.fgb_reference_destroy.restype = None
+    lib.fgb_reference_contigs.argtypes = [vp]
+    lib.fgb_reference_contigs.restype = u64
+    lib.fgb_reference_contig.argtypes = [vp, u64, C.POINTER(C.c_char_p), C.POINTER(u64)]
+    lib.fgb_reference_contig.restype = C.c_int32
+    lib.fgb_filter_records.argtypes = [vp, C.POINTER(FgbRecordFilterOptions), vp, C.c_char_p, C.c_size_t, vp, vp, u64,
+                                       C.POINTER(vp), C.POINTER(u64), C.POINTER(vp), C.POINTER(u64), vp,
+                                       C.POINTER(u64)]
+    lib.fgb_filter_records.restype = C.c_int32
+    lib.fgb_filter_last_timing.argtypes = [vp, vp]
+    lib.fgb_filter_last_timing.restype = C.c_int32
     lib.fgb_struct_size.argtypes = [C.c_uint32]
     lib.fgb_struct_size.restype = C.c_uint32
     _lib = lib

@@ -1126,11 +1126,62 @@ fgb_status fgb_host_sort_verify(const fgb_sort_options* opt, const char* header_
  * [1]-[3]), [4] download, [5] host merge (0 for one run). */
 fgb_status fgb_sort_last_timing(const fgb_handle* h, double ms[6]);
 
+/* ---- `fgumi filter --ref` on raw records (src/lib/commands/filter.rs:550-905): mapped consensus reads masked, their
+ * NM / UQ / MD regenerated against the reference (fgumi-sam alignment_tags.rs:254-420) and the reads or templates that
+ * fail the read-level gates moved to a rejects stream.  Methylation options and compressed FASTA are not offered. */
+typedef struct fgb_reference fgb_reference;
+/* Parses an uncompressed FASTA image (`len` bytes) on the host as the reference's sequential reader does -- a contig's
+ * name runs from after '>' to the first whitespace, its sequence is every following line up to the next '>' with the
+ * line ends (\n, \r\n) removed and the bytes kept as they are -- and uploads the sequence once, as one byte array plus
+ * a contig table, to `device`, where it stays until fgb_reference_destroy.  A gzip / BGZF image or text before the
+ * first '>' gives FGB_ERR_INVALID_ARG; of two contigs with one name the later one is looked up, as in the reference.
+ * device == FGB_DEVICE_NONE parses only: the contig query works, fgb_filter_records refuses it. */
+fgb_status fgb_reference_create(int device, const uint8_t* fasta, size_t len, fgb_reference** out);
+void fgb_reference_destroy(fgb_reference* r);
+/* The contig count; with i < count, contig i's name (NUL-terminated, valid until destroy) and length. */
+uint64_t fgb_reference_contigs(const fgb_reference* r);
+fgb_status fgb_reference_contig(const fgb_reference* r, uint64_t i, const char** name, uint64_t* length);
+
+typedef struct fgb_record_filter_options {
+  fgb_duplex_filter_params filter;   /* the thresholds: cc for simplex reads, cc / ab / ba for duplex ones      */
+  uint8_t filter_by_template;        /* 1: template mode (the default of `fgumi filter`); 0: each record alone    */
+  uint8_t reverse_per_base_tags;     /* --reverse-per-base-tags                                                 */
+  uint8_t track_rejects;             /* 1: rejected records go to the rejects stream                           */
+  uint8_t reserved[1];
+  uint32_t n_threads;                /* host threads (staging copies, templates); 0 or 1 = the calling thread   */
+  uint64_t device_bytes;             /* device-memory budget of one run of templates; 0 = from cudaMemGetInfo   */
+} fgb_record_filter_options;
+enum { FGB_FSTAT_TOTAL = 0, FGB_FSTAT_PASSED = 1, FGB_FSTAT_FAILED = 2, FGB_FSTAT_BASES_MASKED = 3, FGB_FILTER_NSTATS = 4 };
+/* Filters n_records records (record i = records[rec_off[i] .. rec_off[i+1]), no block_size prefix; a call holds whole
+ * templates, a template being the records that share a QNAME consecutively).  Per record, in the reference's order:
+ * the per-base tags of a reverse-strand read reversed (optional), masking (duplex reads, with aD or bD, by the three
+ * tiers; others by cc), NM / UQ / MD regenerated when `ref` is given (unmapped: removed; ref_id -1: untouched), then
+ * the read gates.  Template mode keeps a template when it has a primary record and every primary record passes; its
+ * secondary and supplementary records also need to pass themselves.  Output: *kept and *rejects, library-owned
+ * [u32 block_size][record] streams valid until the next call on `h` (records in template order, or input order in
+ * single-read mode; rejects only with track_rejects), and stats[FGB_FSTAT_*].  Synchronous.
+ * Errors fail the call and emit nothing; *bad_record = the first bad record in input order and fgb_last_error says
+ * why: a record shorter than 32 bytes or with truncated fields (FGB_ERR_LAYOUT), a mapped record without `ref`, a
+ * ref_id outside the header's @SQ lines, a negative position on a mapped record, a contig missing from the FASTA, an
+ * alignment past the contig's end, a CIGAR that consumes more bases than l_seq, a template with two primary R1s or R2s
+ * (FGB_ERR_INVALID_ARG). */
+fgb_status fgb_filter_records(fgb_handle* h, const fgb_record_filter_options* opt, const fgb_reference* ref,
+                              const char* header_text, size_t header_len, const uint8_t* records,
+                              const uint64_t* rec_off, uint64_t n_records, const uint8_t** kept, uint64_t* kept_len,
+                              const uint8_t** rejects, uint64_t* rejects_len, uint64_t stats[FGB_FILTER_NSTATS],
+                              uint64_t* bad_record);
+/* Where the last fgb_filter_records on `h` spent its time, in ms, summed over its runs: [0] upload, [1] pass 1 (tags,
+ * masking, NM / UQ / MD sizes, gates), [2] template decision and offset scans, [3] pass 2 (edited records written),
+ * [4] download (with the growth of the output streams), [5] host work (checks, templates, contig table, and every
+ * device and page-locked allocation of the call).  [1]-[3] are CUDA events.  The staging buffers are at most 64 MiB;
+ * the environment variable FGB_FILTER_STAGE_BYTES (at least 4096) lowers that, read on every call. */
+fgb_status fgb_filter_last_timing(const fgb_handle* h, double ms[6]);
+
 /* sizeof() of the ABI structs as this library was compiled, so a binding can check its own layout:
  * 0 fgb_caller_options, 1 fgb_filter_params, 2 fgb_submit_options, 3 fgb_raw_columns,
  * 4 fgb_raw_read, 5 fgb_batch, 6 fgb_codec_params, 7 fgb_params, 8 fgb_duplex_filter_params,
- * 9 fgb_record_columns, 10 fgb_umi_options, 11 fgb_group_options, 12 fgb_sort_options, 13 fgb_dedup_options; 0 for
- * an unknown id. */
+ * 9 fgb_record_columns, 10 fgb_umi_options, 11 fgb_group_options, 12 fgb_sort_options, 13 fgb_dedup_options,
+ * 14 fgb_record_filter_options; 0 for an unknown id. */
 uint32_t fgb_struct_size(uint32_t id);
 
 #ifdef __cplusplus

@@ -76,5 +76,25 @@ test_bgzf_members_inflated_on_the_device()
 layout, raw = fg.pack_raw_reads([[(b"ACGTNACGTACGTTTGA", bytes(range(5, 22)), bool(i & 1), 17 - (i % 3))] * (1 + i % 4) for i in range(200)], 1, 10)
 o = fg.HostColumns.alloc(layout.n_out)
 eng.submit_bam4(layout, raw, o); eng.wait()
+# record filter: pass 1, decision, scans and pass 2 against the oracle (both modes, tag reversal, rejects)
+import tempfile
+from fgumi_b200 import filter as F
+from tests import filter_oracle as FO, filter_streams as FS
+contigs = FS.genome(3)
+with tempfile.TemporaryDirectory() as d:
+    with open(os.path.join(d, "g.fa"), "wb") as f:
+        f.write(FS.fasta(contigs))
+    ref = F.Reference(os.path.join(d, "g.fa"))
+recs = FS.records(4, contigs, n_templates=120)
+fb, foff = FS.pack(recs)
+for tmpl in (True, False):
+    rf = F.RecordFilter(filter_by_template=tmpl, reverse_per_base_tags=True, track_rejects=True,
+                        max_no_call_fraction=0.5, max_base_error_rate=(0.3,))
+    assert rf.filter(FS.header(contigs), fb, foff, ref) == FO.filter_records(
+        recs, FS.header(contigs), FO.Config(filter_by_template=tmpl, reverse_per_base_tags=True,
+                                            max_no_call_fraction=0.5, max_base_error_rate=(0.3,)),
+        FO.parse_fasta(FS.fasta(contigs)))
+    rf.close()
+ref.close()
 eng.close()
 print("sanitize run ok")
