@@ -92,6 +92,22 @@ def output_header(input_text: bytes, read_group_id: str, command_line: str = "fg
     return ("\n".join(out) + "\n").encode()
 
 
+def _write_bgzf(f, payload, level: int, n_threads: int, eof: bool = True) -> int:
+    """payload (bytes, bytearray or a uint8 array) as BGZF members, with the EOF member when eof, written to the open
+    file f; returns the compressed length."""
+    lib = _l.load()
+    src = np.frombuffer(payload, dtype=np.uint8)
+    cap = lib.fgb_bgzf_bound(len(src))
+    comp = np.empty(max(cap, 1), dtype=np.uint8)
+    cn = C.c_size_t()
+    st = lib.fgb_bgzf_compress(src.ctypes.data, len(src), level, n_threads, int(eof), comp.ctypes.data, cap,
+                               C.addressof(cn))
+    if st != 0:
+        raise _l.FgbError(st, "fgb_bgzf_compress")
+    f.write(comp[:cn.value])
+    return cn.value
+
+
 def simplex_file(in_path: str, out_path: str, caller, n_threads: int = 4, level: int = 1) -> Dict[str, float]:
     """One file-level run with an existing VanillaUmiConsensusCaller (its options decide everything else)."""
     lib = _l.load()
@@ -117,18 +133,13 @@ def simplex_file(in_path: str, out_path: str, caller, n_threads: int = 4, level:
     payload[:hn.value] = hdr[:hn.value]
     if n.value:
         C.memmove(payload.ctypes.data + hn.value, data.value, n.value)
-    cap = lib.fgb_bgzf_bound(len(payload))
-    comp = np.empty(cap, dtype=np.uint8)
-    cn = C.c_size_t()
     t3 = time.perf_counter()
-    st = lib.fgb_bgzf_compress(payload.ctypes.data, len(payload), level, n_threads, 1, comp.ctypes.data, cap, C.addressof(cn))
-    if st != 0:
-        raise _l.FgbError(st, "fgb_bgzf_compress")
+    with open(out_path, "wb") as f:
+        cn = _write_bgzf(f, payload, level, n_threads)
     t4 = time.perf_counter()
-    comp[:cn.value].tofile(out_path)
     tm.update({"group_s": t1 - t0, "caller_s": t2 - t1, "deflate_s": t4 - t3, "input_records": float(len(rec_off) - 1),
                "groups": float(len(groups) - 1), "consensus_reads": float(cnt.value), "output_bytes": float(len(payload)),
-               "output_compressed_bytes": float(cn.value)})
+               "output_compressed_bytes": float(cn)})
     return tm
 
 
@@ -171,21 +182,15 @@ def sort_header(input_text: bytes, order: str, command_line: str = "fgumi_b200 s
 def sort_file(in_path: str, out_path: str, sorter, n_threads: int = 4, level: int = 1) -> Dict[str, float]:
     """`fgumi sort -i in.bam -o out.bam --order <sorter's order>` with an existing sort.RecordSorter.  Returns the
     phase timings: read / inflate / split (read_bam), device (the sort call, with the sorter's own phases), compress."""
-    lib = _l.load()
     text, bodies, rec_off, tm = read_bam(in_path, n_threads)
     t0 = time.perf_counter()
     stream = sorter.sort(text, bodies, rec_off)
     t1 = time.perf_counter()
     payload = mapped_bam_header(sort_header(text, sorter.order)) + stream
-    cap = lib.fgb_bgzf_bound(len(payload))
-    comp = np.empty(cap, dtype=np.uint8)
-    cn = C.c_size_t()
     t2 = time.perf_counter()
-    st = lib.fgb_bgzf_compress(payload, len(payload), level, n_threads, 1, comp.ctypes.data, cap, C.addressof(cn))
-    if st != 0:
-        raise _l.FgbError(st, "fgb_bgzf_compress")
+    with open(out_path, "wb") as f:
+        _write_bgzf(f, payload, level, n_threads)
     t3 = time.perf_counter()
-    comp[:cn.value].tofile(out_path)
     tm.update({"device_s": t1 - t0, "compress_s": t3 - t2, "input_records": float(len(rec_off) - 1),
                "output_bytes": float(len(payload))})
     tm.update({k: v for k, v in sorter.last_timing().items()})
@@ -232,20 +237,14 @@ def group_records(text: bytes, bodies: np.ndarray, rec_off: np.ndarray, grouper,
 def group_file(in_path: str, out_path: str, grouper, n_threads: int = 4, level: int = 1,
                cell_tag: bytes = b"CB") -> Dict[str, float]:
     """`fgumi group -i mapped.bam -o grouped.bam` with an existing ReadGrouper (its options decide the rest)."""
-    lib = _l.load()
     text, bodies, rec_off, tm = read_bam(in_path, n_threads)
     check_group_sort_order(text, grouper.opt.umi.rules == _l.FGB_UMI_RULES_UNMAPPED)
     t0 = time.perf_counter()
     stream = group_records(text, bodies, rec_off, grouper, cell_tag)
     t1 = time.perf_counter()
     payload = mapped_bam_header(group_header(text)) + stream
-    cap = lib.fgb_bgzf_bound(len(payload))
-    comp = np.empty(cap, dtype=np.uint8)
-    cn = C.c_size_t()
-    st = lib.fgb_bgzf_compress(payload, len(payload), level, n_threads, 1, comp.ctypes.data, cap, C.addressof(cn))
-    if st != 0:
-        raise _l.FgbError(st, "fgb_bgzf_compress")
-    comp[:cn.value].tofile(out_path)
+    with open(out_path, "wb") as f:
+        _write_bgzf(f, payload, level, n_threads)
     tm.update({"group_s": t1 - t0, "input_records": float(len(rec_off) - 1), "output_bytes": float(len(payload))})
     return tm
 
@@ -265,20 +264,14 @@ def dedup_file(in_path: str, out_path: str, deduper, n_threads: int = 4, level: 
     """`fgumi dedup -i sorted.bam -o deduped.bam` with an existing dedup.Deduper (its options decide the rest).  Like
     the reference (dedup.rs:1167-1179) it raises ValueError after writing the output when secondary or supplementary
     records of this input lack the `tc` tag; the deduper may be reused across inputs."""
-    lib = _l.load()
     text, bodies, rec_off, tm = read_bam(in_path, n_threads)
     missing_before = deduper.stats()["missing_tc_tag"]   # a deduper may have run on other input before
     t0 = time.perf_counter()
     stream = dedup_records(text, bodies, rec_off, deduper, cell_tag)
     t1 = time.perf_counter()
     payload = mapped_bam_header(group_header(text, "fgumi_b200 dedup")) + stream
-    cap = lib.fgb_bgzf_bound(len(payload))
-    comp = np.empty(cap, dtype=np.uint8)
-    cn = C.c_size_t()
-    st = lib.fgb_bgzf_compress(payload, len(payload), level, n_threads, 1, comp.ctypes.data, cap, C.addressof(cn))
-    if st != 0:
-        raise _l.FgbError(st, "fgb_bgzf_compress")
-    comp[:cn.value].tofile(out_path)
+    with open(out_path, "wb") as f:
+        _write_bgzf(f, payload, level, n_threads)
     tm.update({"dedup_s": t1 - t0, "input_records": float(len(rec_off) - 1), "output_bytes": float(len(payload))})
     missing = deduper.stats()["missing_tc_tag"] - missing_before
     if missing:
@@ -354,20 +347,9 @@ def filter_file(in_path: str, out_path: str, record_filter, reference=None, reje
     written before the next, so that the outputs are never held whole.  A failing batch raises with
     record_filter.bad_record set to the index in the whole input."""
     from .filter import filter_stats_text
-    lib = _l.load()
     text, bodies, rec_off, tm = read_bam(in_path, n_threads)
     header = mapped_bam_header(group_header(text, "fgumi_b200 filter"))
     outs = [(open(path, "wb"), header) for path in (out_path, rejects) if path is not None]
-
-    def write(k, payload, eof):
-        cap = lib.fgb_bgzf_bound(len(payload))
-        comp = np.empty(max(cap, 1), dtype=np.uint8)
-        cn = C.c_size_t()
-        st = lib.fgb_bgzf_compress(payload, len(payload), level, n_threads, 1 if eof else 0, comp.ctypes.data, cap,
-                                   C.addressof(cn))
-        if st != 0:
-            raise _l.FgbError(st, "fgb_bgzf_compress")
-        outs[k][0].write(comp[:cn.value].tobytes())
 
     counts = {"total": 0, "passed": 0, "failed": 0, "bases_masked": 0}
     t_filter = out_bytes = 0.0
@@ -386,10 +368,10 @@ def filter_file(in_path: str, out_path: str, record_filter, reference=None, reje
                 counts[k] += c[k]
             out_bytes += len(kept)
             for k, stream in enumerate((kept, rej)[:len(outs)]):
-                write(k, outs[k][1] + stream, False)
+                _write_bgzf(outs[k][0], outs[k][1] + stream, level, n_threads, False)
                 outs[k] = (outs[k][0], b"")   # the header goes with the first batch only
         for k in range(len(outs)):
-            write(k, outs[k][1], True)          # the header of an empty input, and the EOF member
+            _write_bgzf(outs[k][0], outs[k][1], level, n_threads)   # the header of an empty input, and the EOF member
     finally:
         for f, _ in outs:
             f.close()

@@ -28,6 +28,7 @@
 #include "unpack_kernels.cuh"
 #include "host/dedup_device.h"
 #include "host/filter_device.h"
+#include "host/record_link.h"
 #include "host/sort_device.h"
 #include "host/umi_host.h"
 #include <cub/device/device_radix_sort.cuh>
@@ -1722,13 +1723,17 @@ fgb_status fgb_umi_edges(fgb_handle* h, const fgb_umi_options* opt, const uint8_
 
 }  // extern "C"
 
+// ---- the record commands' view of the handle (host/record_link.h) ------------------------------------------------
+fgb::link::HandleInfo fgb::link::info(fgb_handle* h, Command c) {
+  const bool filter = c == Command::kFilter;
+  return HandleInfo{h->device, h->sm_count, h->slots[0].stream, h->submit_pending, &h->last_error,
+                    filter ? h->filter_timing : h->sort_timing, filter ? &h->filter_kept : nullptr,
+                    filter ? &h->filter_rejects : nullptr};
+}
+
 // ---- record sort (sort_kernels.cuh; the driver is host/sort_host.cpp) --------------------------------------------
 namespace fgb {
 namespace sortdev {
-
-HandleInfo info(fgb_handle* h) {
-  return HandleInfo{h->device, h->sm_count, h->slots[0].stream, h->submit_pending, &h->last_error, h->sort_timing};
-}
 
 namespace {
 unsigned blocks(uint32_t n) { return (n + kSortThreads - 1) / kSortThreads; }
@@ -1796,11 +1801,6 @@ cudaError_t gather(const uint8_t* rec, const uint64_t* off, uint64_t base, const
 // ---- record filter (filter_records_kernels.cuh; the driver is host/filter_host.cpp) ---------------------------------
 namespace fgb {
 namespace filterdev {
-
-HandleInfo info(fgb_handle* h) {
-  return HandleInfo{h->device,        h->sm_count,   h->slots[0].stream, h->submit_pending, &h->last_error,
-                    h->filter_timing, &h->filter_kept, &h->filter_rejects};
-}
 
 namespace {
 unsigned warp_grid(uint32_t n, int sm_count) {   // one warp per record, at most 16 CTAs per SM (grid-stride)

@@ -19,6 +19,7 @@
 #include "bam.h"
 #include "dedup_device.h"
 #include "group_rules.h"
+#include "record_link.h"
 #include "umi_host.h"
 
 namespace {
@@ -26,6 +27,7 @@ namespace {
 using fgb::bam::View;
 namespace bam = fgb::bam;
 using namespace fgb::grp;
+using fgb::link::ms_since;
 
 constexpr uint16_t kDuplicate = 0x400;
 
@@ -299,10 +301,6 @@ fgb_status guard(fgb_deduper* d, const char* where, F&& f) {
     d->last_error = std::string(where) + ": " + e.what();
   }
   return FGB_ERR_NOMEM;
-}
-
-double ms_since(std::chrono::steady_clock::time_point t) {
-  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
 }
 
 }  // namespace

@@ -5,12 +5,8 @@
 
 #include <cstddef>
 #include <cstdint>
-#include <string>
-#include <vector>
 
 #include "record_filter.h"
-
-struct fgb_handle;
 
 namespace fgb {
 
@@ -35,18 +31,6 @@ struct FRec {                         // pass 1's result for one record, read by
 };
 
 namespace filterdev {
-
-struct HandleInfo {
-  int device;
-  int sm_count;
-  cudaStream_t stream;
-  bool busy;                     // a submit has not been waited on
-  std::string* last_error;
-  double* timing;                // fgb_filter_last_timing's six phases
-  std::vector<uint8_t>* kept;    // the library-owned output streams
-  std::vector<uint8_t>* rejects;
-};
-HandleInfo info(fgb_handle* h);
 
 cudaError_t pass1(uint8_t* rec, const uint64_t* off, uint64_t base, uint32_t n, const FilterCfg& cfg,
                   const int32_t* ctg_of_ref, const uint64_t* ctg_off, const uint64_t* ctg_len, const uint8_t* genome,

@@ -20,6 +20,7 @@
 #include "bam.h"
 #include "filter_device.h"
 #include "group_rules.h"
+#include "record_link.h"
 #include "umi_host.h"
 
 struct fgb_reference {
@@ -35,12 +36,9 @@ struct fgb_reference {
 namespace {
 
 namespace dev = fgb::filterdev;
+namespace link = fgb::link;
+using link::ms_since;
 constexpr uint64_t kNone = UINT64_MAX;
-constexpr uint64_t kStageBytes = 64ull << 20;   // one page-locked staging buffer (two alternate)
-
-double ms_since(std::chrono::steady_clock::time_point t) {
-  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
-}
 
 // The sequential FASTA reader's records (reference.rs:229-244): name up to the first whitespace after '>', sequence
 // = the following lines up to the next '>' with \n / \r\n removed.  false: not a FASTA image.
@@ -95,94 +93,6 @@ std::vector<std::string> sq_names(std::string_view text) {
   return out;
 }
 
-// memcpy on n_threads host threads (the staging copies are what bounds the upload and download)
-void par_copy(uint8_t* dst, const uint8_t* src, uint64_t n, uint32_t n_threads) {
-  const uint64_t t = std::min<uint64_t>(std::max<uint32_t>(n_threads, 1), std::max<uint64_t>(n >> 22, 1));
-  fgb_umi::parallel_for(t, n_threads, [&](uint64_t w) {
-    const uint64_t b = n * w / t, e = n * (w + 1) / t;
-    if (e > b) std::memcpy(dst + b, src + b, e - b);
-  });
-}
-
-struct Driver {
-  dev::HandleInfo hi;
-  uint32_t threads;
-  std::vector<void*> dmem;
-  uint8_t* stage[2] = {nullptr, nullptr};
-  cudaEvent_t staged[2] = {nullptr, nullptr};
-  uint64_t stage_bytes = 0;
-  cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  ~Driver() {
-    for (void* p : dmem) cudaFree(p);
-    for (auto* s : stage) if (s) cudaFreeHost(s);
-    for (auto e : staged) if (e) cudaEventDestroy(e);
-    for (auto e : ev) if (e) cudaEventDestroy(e);
-  }
-  template <class T>
-  cudaError_t alloc(T** p, uint64_t count) {
-    void* q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, std::max<uint64_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) dmem.push_back(q);
-    *p = static_cast<T*>(q);
-    return e;
-  }
-  template <class T>
-  cudaError_t grow(T** p, uint64_t* cap, uint64_t count) {   // a buffer of at least `count` elements
-    if (count <= *cap) return cudaSuccess;
-    if (*p) { dmem.erase(std::find(dmem.begin(), dmem.end(), static_cast<void*>(*p))); cudaFree(*p); *p = nullptr; }
-    *cap = 0;
-    const uint64_t want = count + count / 8 + 64;
-    const cudaError_t e = alloc(p, want);
-    if (e == cudaSuccess) *cap = want;
-    return e;
-  }
-  fgb_status fail(cudaError_t e, const char* what) {
-    cudaGetLastError();   // a failed allocation must not surface in the handle's next launch check
-    *hi.last_error = std::string("fgb_filter_records: ") + what + ": " + cudaGetErrorString(e);
-    return e == cudaErrorMemoryAllocation ? FGB_ERR_NOMEM : FGB_ERR_CUDA;
-  }
-  // host -> device through the two staging buffers: the copy into one overlaps the transfer out of the other
-  cudaError_t upload(void* dst_v, const void* src_v, uint64_t n) {
-    uint8_t* dst = static_cast<uint8_t*>(dst_v);
-    const uint8_t* src = static_cast<const uint8_t*>(src_v);
-    for (uint64_t at = 0, k = 0; at < n; at += stage_bytes, ++k) {
-      const int b = static_cast<int>(k & 1);
-      const uint64_t len = std::min(stage_bytes, n - at);
-      cudaError_t e = cudaEventSynchronize(staged[b]);
-      if (e != cudaSuccess) return e;
-      par_copy(stage[b], src + at, len, threads);
-      if ((e = cudaMemcpyAsync(dst + at, stage[b], len, cudaMemcpyHostToDevice, hi.stream)) != cudaSuccess) return e;
-      if ((e = cudaEventRecord(staged[b], hi.stream)) != cudaSuccess) return e;
-    }
-    return cudaSuccess;
-  }
-  // device -> host the same way: the transfer into one buffer overlaps the copy out of the other
-  cudaError_t download(uint8_t* dst, const uint8_t* src, uint64_t n) {
-    uint64_t prev_at = 0, prev_len = 0;
-    int prev = -1;
-    for (uint64_t at = 0, k = 0; at < n; at += stage_bytes, ++k) {
-      const int b = static_cast<int>(k & 1);
-      const uint64_t len = std::min(stage_bytes, n - at);
-      cudaError_t e = cudaEventSynchronize(staged[b]);
-      if (e != cudaSuccess) return e;
-      if ((e = cudaMemcpyAsync(stage[b], src + at, len, cudaMemcpyDeviceToHost, hi.stream)) != cudaSuccess ||
-          (e = cudaEventRecord(staged[b], hi.stream)) != cudaSuccess)
-        return e;
-      if (prev >= 0) {
-        if ((e = cudaEventSynchronize(staged[prev])) != cudaSuccess) return e;
-        par_copy(dst + prev_at, stage[prev], prev_len, threads);
-      }
-      prev = b; prev_at = at; prev_len = len;
-    }
-    if (prev >= 0) {
-      const cudaError_t e = cudaEventSynchronize(staged[prev]);
-      if (e != cudaSuccess) return e;
-      par_copy(dst + prev_at, stage[prev], prev_len, threads);
-    }
-    return cudaSuccess;
-  }
-};
-
 // The checks that need only a record's fixed fields (regenerate_alignment_tags_raw's, alignment_tags.rs:259-291, and
 // the command's no-reference check, commands/filter.rs:758-768): "" or why record i fails the call; *layout: the
 // record is cut short.
@@ -201,11 +111,12 @@ std::string host_check(const uint8_t* r, uint64_t len, bool have_ref, uint64_t n
   return "";
 }
 
-fgb_status filter_impl(fgb_handle* h, const fgb_record_filter_options& o, const fgb_reference* ref,
+fgb_status filter_impl(const link::HandleInfo& hi, const fgb_record_filter_options& o, const fgb_reference* ref,
                        std::string_view header, const uint8_t* records, const uint64_t* rec_off, uint64_t n,
                        uint64_t* stats, uint64_t* bad_record) {
-  Driver d{dev::info(h), std::max<uint32_t>(o.n_threads, 1)};
-  double* tm = d.hi.timing;
+  auto fail = [&](cudaError_t e, const char* what) { return link::fail(hi.last_error, "fgb_filter_records", e, what); };
+  link::Resources r(hi.stream, o.n_threads);
+  double* tm = hi.timing;
   auto t_host = std::chrono::steady_clock::now();
   // header-level checks: the first failing record in input order
   const std::vector<std::string> sq = sq_names(header);
@@ -275,15 +186,11 @@ fgb_status filter_impl(fgb_handle* h, const fgb_record_filter_options& o, const 
       const auto it = ref->index.find(sq[s]);
       if (it != ref->index.end()) ctg[s] = static_cast<int32_t>(it->second);
     }
-  cudaError_t e = cudaSetDevice(d.hi.device);
-  if (e != cudaSuccess) return d.fail(e, "cudaSetDevice");
+  cudaError_t e = cudaSetDevice(hi.device);
+  if (e != cudaSuccess) return fail(e, "cudaSetDevice");
   // runs of whole templates: input bytes, their edited copies in both streams and ~100 bytes of tables per record
-  uint64_t budget = o.device_bytes;
-  if (!budget) {
-    size_t free_b = 0, total_b = 0;
-    if ((e = cudaMemGetInfo(&free_b, &total_b)) != cudaSuccess) return d.fail(e, "cudaMemGetInfo");
-    budget = free_b - free_b / 8 - std::min<uint64_t>(free_b / 8, 512ull << 20);
-  }
+  uint64_t budget;
+  if ((e = link::device_budget(o.device_bytes, &budget)) != cudaSuccess) return fail(e, "cudaMemGetInfo");
   std::vector<uint64_t> run_tpl{0};
   uint64_t max_n = 0, max_bytes = 0;
   for (uint64_t t = 0; t < n_tpl;) {
@@ -310,28 +217,21 @@ fgb_status filter_impl(fgb_handle* h, const fgb_record_filter_options& o, const 
   uint64_t cap_kept = 0, cap_rej = 0;
   size_t t_scan = 0;
   const uint32_t mn = static_cast<uint32_t>(max_n);
-  if ((e = dev::offsets(nullptr, &t_scan, nullptr, nullptr, mn, false, nullptr, nullptr, nullptr, nullptr, d.hi.stream)))
-    return d.fail(e, "CUB temp storage");
-  if ((e = d.alloc(&d_rec, max_bytes + 16)) || (e = d.alloc(&d_off, max_n + 1)) || (e = d.alloc(&d_fr, max_n)) ||
-      (e = d.alloc(&d_order, max_n)) || (e = d.alloc(&d_tpl, max_n + 1)) || (e = d.alloc(&d_ks, max_n + 1)) ||
-      (e = d.alloc(&d_rs, max_n + 1)) || (e = d.alloc(&d_koff, max_n + 1)) || (e = d.alloc(&d_roff, max_n + 1)) ||
-      (e = d.alloc(&d_ctg, ctg.size())) || (e = d.alloc(&d_cnt, 3)) || (e = d.alloc(&d_temp, t_scan + 16)))
-    return d.fail(e, "cudaMalloc");
+  if ((e = dev::offsets(nullptr, &t_scan, nullptr, nullptr, mn, false, nullptr, nullptr, nullptr, nullptr, hi.stream)))
+    return fail(e, "CUB temp storage");
+  if ((e = r.alloc(&d_rec, max_bytes + 16)) || (e = r.alloc(&d_off, max_n + 1)) || (e = r.alloc(&d_fr, max_n)) ||
+      (e = r.alloc(&d_order, max_n)) || (e = r.alloc(&d_tpl, max_n + 1)) || (e = r.alloc(&d_ks, max_n + 1)) ||
+      (e = r.alloc(&d_rs, max_n + 1)) || (e = r.alloc(&d_koff, max_n + 1)) || (e = r.alloc(&d_roff, max_n + 1)) ||
+      (e = r.alloc(&d_ctg, ctg.size())) || (e = r.alloc(&d_cnt, 3)) || (e = r.alloc(&d_temp, t_scan + 16)))
+    return fail(e, "cudaMalloc");
   // FGB_FILTER_STAGE_BYTES (at least 4096) lowers the staging buffers' size, so that small inputs cross several chunks
-  uint64_t stage_cap = kStageBytes;
+  uint64_t stage_cap = link::kStageBytes;
   if (const char* env = std::getenv("FGB_FILTER_STAGE_BYTES"))
-    stage_cap = std::max<uint64_t>(4096, std::min<uint64_t>(kStageBytes, std::strtoull(env, nullptr, 10)));
-  const uint64_t stage = std::min<uint64_t>(stage_cap, std::max<uint64_t>(max_bytes + 64, (max_n + 1) * 8));
-  d.stage_bytes = stage;
-  for (int b = 0; b < 2; ++b) {
-    if ((e = cudaHostAlloc(reinterpret_cast<void**>(&d.stage[b]), stage, cudaHostAllocDefault)) != cudaSuccess)
-      return d.fail(e, "cudaHostAlloc");
-    if ((e = cudaEventCreateWithFlags(&d.staged[b], cudaEventDisableTiming)) != cudaSuccess)
-      return d.fail(e, "cudaEventCreate");
-  }
-  for (auto& x : d.ev)
-    if ((e = cudaEventCreate(&x)) != cudaSuccess) return d.fail(e, "cudaEventCreate");
-  if ((e = cudaMemcpy(d_ctg, ctg.data(), ctg.size() * 4, cudaMemcpyHostToDevice))) return d.fail(e, "cudaMemcpy");
+    stage_cap = std::max<uint64_t>(4096, std::min<uint64_t>(link::kStageBytes, std::strtoull(env, nullptr, 10)));
+  const char* what;
+  if ((e = r.open(std::min<uint64_t>(stage_cap, std::max<uint64_t>(max_bytes + 64, (max_n + 1) * 8)), &what)))
+    return fail(e, what);
+  if ((e = cudaMemcpy(d_ctg, ctg.data(), ctg.size() * 4, cudaMemcpyHostToDevice))) return fail(e, "cudaMemcpy");
   tm[5] += ms_since(t_host);   // host work: the checks, templates and contig table, and every allocation of the call
   fgb::FilterCfg cfg{};
   const fgb_duplex_filter_params& p = o.filter;
@@ -344,8 +244,8 @@ fgb_status filter_impl(fgb_handle* h, const fgb_record_filter_options& o, const 
   cfg.require_ss = p.require_ss_agreement;
   cfg.reverse_tags = o.reverse_per_base_tags;
   cfg.regenerate = ref != nullptr;
-  std::vector<uint8_t>& kept = *d.hi.kept;
-  std::vector<uint8_t>& rej = *d.hi.rejects;
+  std::vector<uint8_t>& kept = *hi.kept;
+  std::vector<uint8_t>& rej = *hi.rejects;
   const bool track = o.track_rejects != 0;
   uint64_t masked = 0, passed = 0;
   std::vector<uint32_t> lorder, ltpl;
@@ -364,37 +264,37 @@ fgb_status filter_impl(fgb_handle* h, const fgb_record_filter_options& o, const 
     const uint64_t base = rec_off[rb], bytes = rec_off[rb + nr] - base;
     auto t_up = std::chrono::steady_clock::now();
     const unsigned long long init[3] = {0, 0, ~0ull};
-    if ((e = d.upload(d_rec, records + base, bytes)) || (e = d.upload(d_off, rec_off + rb, (nr64 + 1) * 8)) ||
-        (e = d.upload(d_order, lorder.data(), nr64 * 4)) || (e = d.upload(d_tpl, ltpl.data(), ltpl.size() * 4)) ||
-        (e = cudaMemcpyAsync(d_cnt, init, sizeof(init), cudaMemcpyHostToDevice, d.hi.stream)) ||
-        (e = cudaStreamSynchronize(d.hi.stream)))
-      return d.fail(e, "upload");
+    if ((e = r.upload(d_rec, records + base, bytes)) || (e = r.upload(d_off, rec_off + rb, (nr64 + 1) * 8)) ||
+        (e = r.upload(d_order, lorder.data(), nr64 * 4)) || (e = r.upload(d_tpl, ltpl.data(), ltpl.size() * 4)) ||
+        (e = cudaMemcpyAsync(d_cnt, init, sizeof(init), cudaMemcpyHostToDevice, hi.stream)) ||
+        (e = cudaStreamSynchronize(hi.stream)))
+      return fail(e, "upload");
     tm[0] += ms_since(t_up);
     uint64_t tot[2];
     unsigned long long cnt[3];
     size_t tb = t_scan + 16;
-    if ((e = cudaEventRecord(d.ev[0], d.hi.stream)) ||
+    if ((e = cudaEventRecord(r.ev[0], hi.stream)) ||
         (e = dev::pass1(d_rec, d_off, base, nr, cfg, d_ctg, d_ctg_off, d_ctg_len, ref ? ref->d_seq : nullptr, rb, d_fr,
-                        d_cnt + 2, d_cnt, d.hi.sm_count, d.hi.stream)) ||
-        (e = cudaEventRecord(d.ev[1], d.hi.stream)) ||
+                        d_cnt + 2, d_cnt, hi.sm_count, hi.stream)) ||
+        (e = cudaEventRecord(r.ev[1], hi.stream)) ||
         (e = dev::decide(d_fr, d_order, d_tpl, static_cast<uint32_t>(t1 - t0), o.filter_by_template != 0, d_cnt,
-                         d.hi.stream)) ||
-        (e = dev::offsets(d_temp, &tb, d_fr, d_order, nr, track, d_ks, d_rs, d_koff, d_roff, d.hi.stream)) ||
-        (e = cudaEventRecord(d.ev[2], d.hi.stream)) ||
-        (e = cudaMemcpyAsync(&tot[0], d_koff + nr, 8, cudaMemcpyDeviceToHost, d.hi.stream)) ||
-        (e = cudaMemcpyAsync(&tot[1], d_roff + nr, 8, cudaMemcpyDeviceToHost, d.hi.stream)) ||
-        (e = cudaMemcpyAsync(cnt, d_cnt, sizeof(cnt), cudaMemcpyDeviceToHost, d.hi.stream)) ||
-        (e = cudaStreamSynchronize(d.hi.stream)))
-      return d.fail(e, "pass 1");
+                         hi.stream)) ||
+        (e = dev::offsets(d_temp, &tb, d_fr, d_order, nr, track, d_ks, d_rs, d_koff, d_roff, hi.stream)) ||
+        (e = cudaEventRecord(r.ev[2], hi.stream)) ||
+        (e = cudaMemcpyAsync(&tot[0], d_koff + nr, 8, cudaMemcpyDeviceToHost, hi.stream)) ||
+        (e = cudaMemcpyAsync(&tot[1], d_roff + nr, 8, cudaMemcpyDeviceToHost, hi.stream)) ||
+        (e = cudaMemcpyAsync(cnt, d_cnt, sizeof(cnt), cudaMemcpyDeviceToHost, hi.stream)) ||
+        (e = cudaStreamSynchronize(hi.stream)))
+      return fail(e, "pass 1");
     if (cnt[2] != ~0ull) {   // a device error: before the first host error by construction
       const uint64_t bi = cnt[2] >> 8;
       const uint8_t code = static_cast<uint8_t>(cnt[2] & 0xFF);
       const int32_t rid = fgb::bam::rdi32(records + rec_off[bi]);
       *bad_record = bi;
-      *d.hi.last_error = "fgb_filter_records: record " + std::to_string(bi) + " " +
-                         (code == fgb::kErrContig   ? "is aligned to reference sequence '" + sq[rid] + "', which the FASTA lacks"
-                          : code == fgb::kErrPastEnd ? "is aligned past the end of reference sequence '" + sq[rid] + "'"
-                                                     : std::string("has a CIGAR that consumes more bases than its sequence"));
+      *hi.last_error = "fgb_filter_records: record " + std::to_string(bi) + " " +
+                       (code == fgb::kErrContig   ? "is aligned to reference sequence '" + sq[rid] + "', which the FASTA lacks"
+                        : code == fgb::kErrPastEnd ? "is aligned past the end of reference sequence '" + sq[rid] + "'"
+                                                   : std::string("has a CIGAR that consumes more bases than its sequence"));
       kept.clear();
       rej.clear();
       return FGB_ERR_INVALID_ARG;
@@ -402,30 +302,30 @@ fgb_status filter_impl(fgb_handle* h, const fgb_record_filter_options& o, const 
     masked += cnt[0];
     passed += cnt[1];
     t_host = std::chrono::steady_clock::now();
-    if ((e = d.grow(&d_kept, &cap_kept, tot[0] + 16)) || (e = d.grow(&d_rej, &cap_rej, tot[1] + 16)))
-      return d.fail(e, "cudaMalloc");
+    if ((e = r.grow(&d_kept, &cap_kept, tot[0] + 16)) || (e = r.grow(&d_rej, &cap_rej, tot[1] + 16)))
+      return fail(e, "cudaMalloc");
     tm[5] += ms_since(t_host);
-    if ((e = cudaEventRecord(d.ev[3], d.hi.stream)) ||
+    if ((e = cudaEventRecord(r.ev[3], hi.stream)) ||
         (e = dev::pass2(d_rec, d_off, base, nr, d_fr, d_order, d_koff, d_roff, track, ref ? ref->d_seq : nullptr,
-                        d_kept, d_rej, d.hi.sm_count, d.hi.stream)) ||
-        (e = cudaEventRecord(d.ev[4], d.hi.stream)) || (e = cudaStreamSynchronize(d.hi.stream)))
-      return d.fail(e, "pass 2");
+                        d_kept, d_rej, hi.sm_count, hi.stream)) ||
+        (e = cudaEventRecord(r.ev[4], hi.stream)) || (e = cudaStreamSynchronize(hi.stream)))
+      return fail(e, "pass 2");
     float a = 0, b = 0, c = 0;
-    cudaEventElapsedTime(&a, d.ev[0], d.ev[1]);
-    cudaEventElapsedTime(&b, d.ev[1], d.ev[2]);
-    cudaEventElapsedTime(&c, d.ev[3], d.ev[4]);
+    cudaEventElapsedTime(&a, r.ev[0], r.ev[1]);
+    cudaEventElapsedTime(&b, r.ev[1], r.ev[2]);
+    cudaEventElapsedTime(&c, r.ev[3], r.ev[4]);
     tm[1] += a; tm[2] += b; tm[3] += c;
     auto t_dn = std::chrono::steady_clock::now();
     const uint64_t k0 = kept.size(), j0 = rej.size();
     kept.resize(k0 + tot[0]);
     rej.resize(j0 + tot[1]);
-    if ((e = d.download(kept.data() + k0, d_kept, tot[0])) || (e = d.download(rej.data() + j0, d_rej, tot[1])))
-      return d.fail(e, "download");
+    if ((e = r.download(kept.data() + k0, d_kept, tot[0])) || (e = r.download(rej.data() + j0, d_rej, tot[1])))
+      return fail(e, "download");
     tm[4] += ms_since(t_dn);
   }
   if (hb < n) {
     *bad_record = hb;
-    *d.hi.last_error = "fgb_filter_records: record " + std::to_string(hb) + " " + herr;
+    *hi.last_error = "fgb_filter_records: record " + std::to_string(hb) + " " + herr;
     kept.clear();
     rej.clear();
     return hst;
@@ -504,7 +404,7 @@ fgb_status fgb_filter_records(fgb_handle* h, const fgb_record_filter_options* op
   if (!h || !opt || !kept || !kept_len || !rejects || !rejects_len || !stats || !rec_off ||
       (n_records && !records) || (header_len && !header_text))
     return FGB_ERR_INVALID_ARG;
-  const dev::HandleInfo hi = dev::info(h);
+  const link::HandleInfo hi = link::info(h, link::Command::kFilter);
   uint64_t bad = kNone;
   std::fill(hi.timing, hi.timing + 6, 0.0);
   std::fill(stats, stats + FGB_FILTER_NSTATS, 0);
@@ -515,20 +415,13 @@ fgb_status fgb_filter_records(fgb_handle* h, const fgb_record_filter_options* op
     return FGB_ERR_INVALID_ARG;
   }
   if (hi.busy) { *hi.last_error = "fgb_filter_records: a submit has not been waited on"; return FGB_ERR_BUSY; }
-  fgb_status st;
-  try {
+  const fgb_status st = link::guarded(hi, "fgb_filter_records", [&]() -> fgb_status {
     hi.kept->clear();
     hi.rejects->clear();
-    st = n_records ? filter_impl(h, *opt, ref, std::string_view(header_text ? header_text : "", header_len), records,
-                                 rec_off, n_records, stats, &bad)
-                   : FGB_OK;
-  } catch (const std::bad_alloc&) {
-    *hi.last_error = "fgb_filter_records: out of host memory";
-    st = FGB_ERR_NOMEM;
-  } catch (const std::exception& x) {
-    *hi.last_error = std::string("fgb_filter_records: ") + x.what();
-    st = FGB_ERR_NOMEM;
-  }
+    return n_records ? filter_impl(hi, *opt, ref, std::string_view(header_text ? header_text : "", header_len), records,
+                                   rec_off, n_records, stats, &bad)
+                     : FGB_OK;
+  });
   if (bad_record) *bad_record = bad;
   if (st != FGB_OK) {
     hi.kept->clear();
@@ -545,7 +438,7 @@ fgb_status fgb_filter_records(fgb_handle* h, const fgb_record_filter_options* op
 
 fgb_status fgb_filter_last_timing(const fgb_handle* h, double ms[6]) {
   if (!h || !ms) return FGB_ERR_INVALID_ARG;
-  std::memcpy(ms, dev::info(const_cast<fgb_handle*>(h)).timing, 6 * sizeof(double));
+  std::memcpy(ms, link::info(const_cast<fgb_handle*>(h), link::Command::kFilter).timing, 6 * sizeof(double));
   return FGB_OK;
 }
 

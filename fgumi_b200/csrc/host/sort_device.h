@@ -5,24 +5,11 @@
 
 #include <cstddef>
 #include <cstdint>
-#include <string>
 
 #include "../sort_keys.h"
 
-struct fgb_handle;
-
 namespace fgb {
 namespace sortdev {
-
-struct HandleInfo {
-  int device;
-  int sm_count;
-  cudaStream_t stream;
-  bool busy;                 // a submit has not been waited on
-  std::string* last_error;
-  double* timing;            // fgb_sort_last_timing's six phases
-};
-HandleInfo info(fgb_handle* h);
 
 // Key words (SoA, `words` of them: 1 for coordinate, 5 for template-coordinate), record sizes and the AND / OR of each
 // word over the run, which `and_or` must hold as (~0, 0) pairs on entry.

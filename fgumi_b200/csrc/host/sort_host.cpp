@@ -17,6 +17,7 @@
 #include "../../../include/fgumi_b200.h"
 #include "../sort_keys.h"
 #include "bam.h"
+#include "record_link.h"
 #include "sort_device.h"
 #include "umi_host.h"
 
@@ -24,12 +25,13 @@ namespace {
 
 namespace sk = fgb::sortk;
 namespace dev = fgb::sortdev;
+namespace link = fgb::link;
+using link::ms_since;
 
 static_assert(FGB_SORT_COORDINATE == sk::kCoordinate && FGB_SORT_TEMPLATE_COORDINATE == sk::kTemplateCoordinate &&
                   FGB_SORT_QUERYNAME == sk::kQueryname && FGB_SORT_QUERYNAME_NATURAL == sk::kQuerynameNatural,
               "sort orders");
 constexpr uint64_t kNone = UINT64_MAX;
-constexpr uint64_t kStageBytes = 64ull << 20;   // one page-locked staging buffer (two alternate)
 
 // LibraryLookup::from_header (raw.rs:237-283): the distinct LB values sorted bytewise and numbered from 1; each RG ID
 // maps to its LB's ordinal, an RG without LB to that of "" (0 unless some LB is empty).  IDs are kept sorted bytewise
@@ -110,108 +112,19 @@ void host_keys(const fgb_sort_options& o, std::string_view header, const uint8_t
   });
 }
 
-// memcpy on n_threads host threads (the staging copies are what bounds the upload and download)
-void par_copy(uint8_t* dst, const uint8_t* src, uint64_t n, uint32_t n_threads) {
-  const uint64_t t = std::min<uint64_t>(std::max<uint32_t>(n_threads, 1), std::max<uint64_t>(n >> 22, 1));
-  fgb_umi::parallel_for(t, n_threads, [&](uint64_t w) {
-    const uint64_t b = n * w / t, e = n * (w + 1) / t;
-    if (e > b) std::memcpy(dst + b, src + b, e - b);
-  });
-}
-
-// Everything one fgb_sort_records call allocates, freed on every way out.
-struct Resources {
-  std::vector<void*> dev;
-  uint8_t* stage[2] = {nullptr, nullptr};
-  cudaEvent_t staged[2] = {nullptr, nullptr};
-  cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  ~Resources() {
-    for (void* p : dev) cudaFree(p);
-    for (auto* s : stage) if (s) cudaFreeHost(s);
-    for (auto e : staged) if (e) cudaEventDestroy(e);
-    for (auto e : ev) if (e) cudaEventDestroy(e);
-  }
-  template <class T>
-  cudaError_t alloc(T** p, uint64_t count) {
-    void* q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, std::max<uint64_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) dev.push_back(q);
-    *p = static_cast<T*>(q);
-    return e;
-  }
-};
-
-struct Driver {
-  dev::HandleInfo hi;
-  const fgb_sort_options& o;
-  uint32_t threads;
-  Resources r;
-  cudaStream_t s;
-
-  fgb_status fail(cudaError_t e, const char* what) {
-    cudaGetLastError();   // a failed allocation must not surface in the handle's next launch check
-    *hi.last_error = std::string("fgb_sort_records: ") + what + ": " + cudaGetErrorString(e);
-    return e == cudaErrorMemoryAllocation ? FGB_ERR_NOMEM : FGB_ERR_CUDA;
-  }
-
-  // host -> device through the two staging buffers: the copy into one overlaps the transfer out of the other
-  cudaError_t upload(uint8_t* dst, const uint8_t* src, uint64_t n) {
-    for (uint64_t at = 0, k = 0; at < n; at += kStageBytes, ++k) {
-      const int b = static_cast<int>(k & 1);
-      const uint64_t len = std::min(kStageBytes, n - at);
-      cudaError_t e = cudaEventSynchronize(r.staged[b]);
-      if (e != cudaSuccess) return e;
-      par_copy(r.stage[b], src + at, len, threads);
-      if ((e = cudaMemcpyAsync(dst + at, r.stage[b], len, cudaMemcpyHostToDevice, s)) != cudaSuccess) return e;
-      if ((e = cudaEventRecord(r.staged[b], s)) != cudaSuccess) return e;
-    }
-    return cudaStreamSynchronize(s);
-  }
-
-  // device -> host the same way: the transfer into one buffer overlaps the copy out of the other
-  cudaError_t download(uint8_t* dst, const uint8_t* src, uint64_t n) {
-    uint64_t prev_at = 0, prev_len = 0;
-    int prev = -1;
-    for (uint64_t at = 0, k = 0; at < n; at += kStageBytes, ++k) {
-      const int b = static_cast<int>(k & 1);
-      const uint64_t len = std::min(kStageBytes, n - at);
-      cudaError_t e = cudaMemcpyAsync(r.stage[b], src + at, len, cudaMemcpyDeviceToHost, s);
-      if (e != cudaSuccess || (e = cudaEventRecord(r.staged[b], s)) != cudaSuccess) return e;
-      if (prev >= 0) {
-        if ((e = cudaEventSynchronize(r.staged[prev])) != cudaSuccess) return e;
-        par_copy(dst + prev_at, r.stage[prev], prev_len, threads);
-      }
-      prev = b; prev_at = at; prev_len = len;
-    }
-    if (prev >= 0) {
-      const cudaError_t e = cudaEventSynchronize(r.staged[prev]);
-      if (e != cudaSuccess) return e;
-      par_copy(dst + prev_at, r.stage[prev], prev_len, threads);
-    }
-    return cudaSuccess;
-  }
-};
-
-double ms_since(std::chrono::steady_clock::time_point t) {
-  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
-}
-
-fgb_status sort_impl(fgb_handle* h, const fgb_sort_options& o, std::string_view header, const uint8_t* records,
-                     const uint64_t* rec_off, uint64_t n, uint8_t* out) {
-  Driver d{dev::info(h), o, std::max<uint32_t>(o.n_threads, 1), {}, nullptr};
-  d.s = d.hi.stream;
-  double* tm = d.hi.timing;
+fgb_status sort_impl(const link::HandleInfo& hi, const fgb_sort_options& o, std::string_view header,
+                     const uint8_t* records, const uint64_t* rec_off, uint64_t n, uint8_t* out) {
+  auto fail = [&](cudaError_t e, const char* what) { return link::fail(hi.last_error, "fgb_sort_records", e, what); };
+  link::Resources r(hi.stream, o.n_threads);
+  const cudaStream_t s = hi.stream;
+  double* tm = hi.timing;
   const bool qn = queryname(o), natural = o.order == FGB_SORT_QUERYNAME_NATURAL;
-  cudaError_t e = cudaSetDevice(d.hi.device);
-  if (e != cudaSuccess) return d.fail(e, "cudaSetDevice");
+  cudaError_t e = cudaSetDevice(hi.device);
+  if (e != cudaSuccess) return fail(e, "cudaSetDevice");
   // runs: as many records as fit the budget (input and output bytes, keys, permutations and scan / sort scratch: 68 +
   // 8 W bytes per record, W the run's key words)
-  uint64_t budget = o.device_bytes;
-  if (!budget) {
-    size_t free_b = 0, total_b = 0;
-    if ((e = cudaMemGetInfo(&free_b, &total_b)) != cudaSuccess) return d.fail(e, "cudaMemGetInfo");
-    budget = free_b - free_b / 8 - std::min<uint64_t>(free_b / 8, 512ull << 20);
-  }
+  uint64_t budget;
+  if ((e = link::device_budget(o.device_bytes, &budget)) != cudaSuccess) return fail(e, "cudaMemGetInfo");
   auto lrn = [&](uint64_t i) -> uint32_t { return qn ? records[rec_off[i] + 8] : 0; };   // l_read_name
   std::vector<uint64_t> run_begin{0};
   std::vector<int> run_words;
@@ -245,31 +158,25 @@ fgb_status sort_impl(fgb_handle* h, const fgb_sort_options& o, std::string_view 
   unsigned long long* d_andor;
   const uint32_t mn = static_cast<uint32_t>(max_n);
   size_t t_sort = 0, t_scan = 0;
-  if ((e = dev::radix_pass(nullptr, &t_sort, nullptr, nullptr, nullptr, nullptr, mn, 0, 64, d.s)) != cudaSuccess ||
-      (e = dev::out_offsets(nullptr, &t_scan, nullptr, nullptr, mn, nullptr, nullptr, d.s)) != cudaSuccess)
-    return d.fail(e, "CUB temp storage");
-  if ((e = d.r.alloc(&d_rec, max_bytes + 16)) != cudaSuccess || (e = d.r.alloc(&d_out, max_bytes + 4 * max_n)) ||
-      (e = d.r.alloc(&d_off, max_n + 1)) || (e = d.r.alloc(&d_keys, max_cells)) ||
-      (e = d.r.alloc(&d_ktmp[0], max_n)) || (e = d.r.alloc(&d_ktmp[1], max_n)) ||
-      (e = d.r.alloc(&d_osize, max_n + 1)) || (e = d.r.alloc(&d_ooff, max_n + 1)) || (e = d.r.alloc(&d_size, max_n)) ||
-      (e = d.r.alloc(&d_perm[0], max_n)) || (e = d.r.alloc(&d_perm[1], max_n)) ||
-      (e = d.r.alloc(&d_rg, l.bytes.size())) || (e = d.r.alloc(&d_rgoff, l.off.size())) ||
-      (e = d.r.alloc(&d_rglib, l.lib.size())) || (e = d.r.alloc(&d_andor, 2 * max_words)) ||
-      (e = d.r.alloc(&d_temp, std::max(t_sort, t_scan) + 16)) || (merge_keys && (e = d.r.alloc(&d_rows, max_cells))))
-    return d.fail(e, "cudaMalloc");
-  const uint64_t stage = std::min<uint64_t>(kStageBytes, std::max(max_bytes + 4 * max_n, (max_n + 1) * 8));
-  for (int b = 0; b < 2; ++b) {
-    if ((e = cudaHostAlloc(reinterpret_cast<void**>(&d.r.stage[b]), stage, cudaHostAllocDefault)) != cudaSuccess)
-      return d.fail(e, "cudaHostAlloc");
-    if ((e = cudaEventCreateWithFlags(&d.r.staged[b], cudaEventDisableTiming)) != cudaSuccess)
-      return d.fail(e, "cudaEventCreate");
-  }
-  for (auto& ev : d.r.ev)
-    if ((e = cudaEventCreate(&ev)) != cudaSuccess) return d.fail(e, "cudaEventCreate");
+  if ((e = dev::radix_pass(nullptr, &t_sort, nullptr, nullptr, nullptr, nullptr, mn, 0, 64, s)) != cudaSuccess ||
+      (e = dev::out_offsets(nullptr, &t_scan, nullptr, nullptr, mn, nullptr, nullptr, s)) != cudaSuccess)
+    return fail(e, "CUB temp storage");
+  if ((e = r.alloc(&d_rec, max_bytes + 16)) != cudaSuccess || (e = r.alloc(&d_out, max_bytes + 4 * max_n)) ||
+      (e = r.alloc(&d_off, max_n + 1)) || (e = r.alloc(&d_keys, max_cells)) ||
+      (e = r.alloc(&d_ktmp[0], max_n)) || (e = r.alloc(&d_ktmp[1], max_n)) ||
+      (e = r.alloc(&d_osize, max_n + 1)) || (e = r.alloc(&d_ooff, max_n + 1)) || (e = r.alloc(&d_size, max_n)) ||
+      (e = r.alloc(&d_perm[0], max_n)) || (e = r.alloc(&d_perm[1], max_n)) ||
+      (e = r.alloc(&d_rg, l.bytes.size())) || (e = r.alloc(&d_rgoff, l.off.size())) ||
+      (e = r.alloc(&d_rglib, l.lib.size())) || (e = r.alloc(&d_andor, 2 * max_words)) ||
+      (e = r.alloc(&d_temp, std::max(t_sort, t_scan) + 16)) || (merge_keys && (e = r.alloc(&d_rows, max_cells))))
+    return fail(e, "cudaMalloc");
+  const char* what;
+  if ((e = r.open(std::min<uint64_t>(link::kStageBytes, std::max(max_bytes + 4 * max_n, (max_n + 1) * 8)), &what)))
+    return fail(e, what);
   if ((!l.bytes.empty() && (e = cudaMemcpy(d_rg, l.bytes.data(), l.bytes.size(), cudaMemcpyHostToDevice))) ||
       (e = cudaMemcpy(d_rgoff, l.off.data(), l.off.size() * 4, cudaMemcpyHostToDevice)) ||
       (!l.lib.empty() && (e = cudaMemcpy(d_rglib, l.lib.data(), l.lib.size() * 4, cudaMemcpyHostToDevice))))
-    return d.fail(e, "cudaMemcpy");
+    return fail(e, "cudaMemcpy");
   const sk::Ctx ctx = make_ctx(o, d_rg, d_rgoff, d_rglib, static_cast<uint32_t>(l.lib.size()));
   // several runs: each run's sorted stream and its keys in sorted order (row-major) come back for the merge
   std::vector<uint8_t> run_stream;
@@ -283,57 +190,57 @@ fgb_status sort_impl(fgb_handle* h, const fgb_sort_options& o, std::string_view 
     const int W = run_words[x];
     const uint64_t base = rec_off[b], bytes = rec_off[b + nr64] - base, out_at = base - rec_off[0] + 4 * b;
     auto t0 = std::chrono::steady_clock::now();
-    if ((e = d.upload(d_rec, records + base, bytes)) != cudaSuccess ||
-        (e = d.upload(reinterpret_cast<uint8_t*>(d_off), reinterpret_cast<const uint8_t*>(rec_off + b), (nr64 + 1) * 8)))
-      return d.fail(e, "upload");
+    if ((e = r.upload(d_rec, records + base, bytes)) || (e = r.upload(d_off, rec_off + b, (nr64 + 1) * 8)) ||
+        (e = cudaStreamSynchronize(s)))
+      return fail(e, "upload");
     tm[0] += ms_since(t0);
-    if ((e = cudaMemcpyAsync(d_andor, init.data(), 16 * W, cudaMemcpyHostToDevice, d.s)) ||
-        (e = cudaEventRecord(d.r.ev[0], d.s)) ||
-        (e = qn ? dev::name_keys(d_rec, d_off, base, nr, natural, W - 1, d_keys, d_size, d_andor, d.s)
-                : dev::keys(d_rec, d_off, base, nr, ctx, W, d_keys, d_size, d_andor, d.s)) ||
-        (e = cudaEventRecord(d.r.ev[1], d.s)) ||
-        (e = cudaMemcpyAsync(and_or.data(), d_andor, 16 * W, cudaMemcpyDeviceToHost, d.s)) ||
-        (e = cudaStreamSynchronize(d.s)))
-      return d.fail(e, "key kernel");
+    if ((e = cudaMemcpyAsync(d_andor, init.data(), 16 * W, cudaMemcpyHostToDevice, s)) ||
+        (e = cudaEventRecord(r.ev[0], s)) ||
+        (e = qn ? dev::name_keys(d_rec, d_off, base, nr, natural, W - 1, d_keys, d_size, d_andor, s)
+                : dev::keys(d_rec, d_off, base, nr, ctx, W, d_keys, d_size, d_andor, s)) ||
+        (e = cudaEventRecord(r.ev[1], s)) ||
+        (e = cudaMemcpyAsync(and_or.data(), d_andor, 16 * W, cudaMemcpyDeviceToHost, s)) ||
+        (e = cudaStreamSynchronize(s)))
+      return fail(e, "key kernel");
     // LSD over the words, last first, skipping constant ones and sorting only the bits that vary
     uint32_t* perm = d_perm[0];
     uint32_t* spare = d_perm[1];
     bool first = true;
-    if ((e = cudaEventRecord(d.r.ev[2], d.s)) != cudaSuccess) return d.fail(e, "cudaEventRecord");
+    if ((e = cudaEventRecord(r.ev[2], s)) != cudaSuccess) return fail(e, "cudaEventRecord");
     for (int w = W - 1; w >= 0; --w) {
       const uint64_t diff = and_or[2 * w] ^ and_or[2 * w + 1];
       if (!diff) continue;
-      const int lo = __builtin_ctzll(diff), hi = 64 - __builtin_clzll(diff);
+      const int begin = __builtin_ctzll(diff), end = 64 - __builtin_clzll(diff);
       const uint64_t* src = d_keys + static_cast<uint64_t>(w) * nr;
-      if (first) e = dev::iota(perm, nr, d.s);
-      else { e = dev::word_gather(src, perm, nr, d_ktmp[0], d.s); src = d_ktmp[0]; }
+      if (first) e = dev::iota(perm, nr, s);
+      else { e = dev::word_gather(src, perm, nr, d_ktmp[0], s); src = d_ktmp[0]; }
       size_t tb = std::max(t_sort, t_scan) + 16;
-      if (e || (e = dev::radix_pass(d_temp, &tb, src, d_ktmp[1], perm, spare, nr, lo, hi, d.s)))
-        return d.fail(e, "radix pass");
+      if (e || (e = dev::radix_pass(d_temp, &tb, src, d_ktmp[1], perm, spare, nr, begin, end, s)))
+        return fail(e, "radix pass");
       std::swap(perm, spare);
       first = false;
     }
-    if (first && (e = dev::iota(perm, nr, d.s))) return d.fail(e, "iota");
+    if (first && (e = dev::iota(perm, nr, s))) return fail(e, "iota");
     size_t tb = std::max(t_sort, t_scan) + 16;
-    if ((e = cudaEventRecord(d.r.ev[3], d.s)) ||
-        (e = dev::out_offsets(d_temp, &tb, d_size, perm, nr, d_osize, d_ooff, d.s)) ||
-        (e = dev::gather(d_rec, d_off, base, perm, d_ooff, nr, d_out, d.hi.sm_count, d.s)) ||
-        (merge_keys && (e = dev::key_rows(d_keys, perm, nr, W, d_rows, d.s))) ||
-        (e = cudaEventRecord(d.r.ev[4], d.s)) || (e = cudaStreamSynchronize(d.s)))
-      return d.fail(e, "gather");
+    if ((e = cudaEventRecord(r.ev[3], s)) ||
+        (e = dev::out_offsets(d_temp, &tb, d_size, perm, nr, d_osize, d_ooff, s)) ||
+        (e = dev::gather(d_rec, d_off, base, perm, d_ooff, nr, d_out, hi.sm_count, s)) ||
+        (merge_keys && (e = dev::key_rows(d_keys, perm, nr, W, d_rows, s))) ||
+        (e = cudaEventRecord(r.ev[4], s)) || (e = cudaStreamSynchronize(s)))
+      return fail(e, "gather");
     float k_ms = 0, s_ms = 0, g_ms = 0;
-    cudaEventElapsedTime(&k_ms, d.r.ev[0], d.r.ev[1]);
-    cudaEventElapsedTime(&s_ms, d.r.ev[2], d.r.ev[3]);
-    cudaEventElapsedTime(&g_ms, d.r.ev[3], d.r.ev[4]);
+    cudaEventElapsedTime(&k_ms, r.ev[0], r.ev[1]);
+    cudaEventElapsedTime(&s_ms, r.ev[2], r.ev[3]);
+    cudaEventElapsedTime(&g_ms, r.ev[3], r.ev[4]);
     tm[1] += k_ms; tm[2] += s_ms; tm[3] += g_ms;
     t0 = std::chrono::steady_clock::now();
     const uint64_t out_bytes = bytes + 4 * nr64;
-    if ((e = d.download((n_runs > 1 ? run_stream.data() : out) + out_at, d_out, out_bytes)))
-      return d.fail(e, "download");
+    if ((e = r.download((n_runs > 1 ? run_stream.data() : out) + out_at, d_out, out_bytes)))
+      return fail(e, "download");
     if (merge_keys) {
       run_keys[x].resize(W * nr64);
       if ((e = cudaMemcpy(run_keys[x].data(), d_rows, W * nr64 * 8, cudaMemcpyDeviceToHost)))
-        return d.fail(e, "download");
+        return fail(e, "download");
     }
     tm[4] += ms_since(t0);
   }
@@ -467,7 +374,7 @@ fgb_status fgb_sort_records(fgb_handle* h, const fgb_sort_options* opt, const ch
                             const uint8_t* records, const uint64_t* rec_off, uint64_t n_records, uint8_t* out,
                             uint64_t cap, uint64_t* out_len, uint64_t* bad_record) {
   if (!h || !out_len || !args_ok(opt, header_text, header_len, records, rec_off, n_records)) return FGB_ERR_INVALID_ARG;
-  const dev::HandleInfo hi = dev::info(h);
+  const link::HandleInfo hi = link::info(h, link::Command::kSort);
   if (bad_record) *bad_record = kNone;
   std::fill(hi.timing, hi.timing + 6, 0.0);
   if (!records_ok(rec_off, n_records, bad_record)) {
@@ -482,20 +389,15 @@ fgb_status fgb_sort_records(fgb_handle* h, const fgb_sort_options* opt, const ch
   if (hi.busy) { *hi.last_error = "fgb_sort_records: a submit has not been waited on"; return FGB_ERR_BUSY; }
   *out_len = need;
   if (!n_records) return FGB_OK;
-  try {
-    return sort_impl(h, *opt, std::string_view(header_text ? header_text : "", header_len), records, rec_off,
+  return link::guarded(hi, "fgb_sort_records", [&] {
+    return sort_impl(hi, *opt, std::string_view(header_text ? header_text : "", header_len), records, rec_off,
                      n_records, out);
-  } catch (const std::bad_alloc&) {
-    *hi.last_error = "fgb_sort_records: out of host memory";
-  } catch (const std::exception& x) {
-    *hi.last_error = std::string("fgb_sort_records: ") + x.what();
-  }
-  return FGB_ERR_NOMEM;
+  });
 }
 
 fgb_status fgb_sort_last_timing(const fgb_handle* h, double ms[6]) {
   if (!h || !ms) return FGB_ERR_INVALID_ARG;
-  std::memcpy(ms, dev::info(const_cast<fgb_handle*>(h)).timing, 6 * sizeof(double));
+  std::memcpy(ms, link::info(const_cast<fgb_handle*>(h), link::Command::kSort).timing, 6 * sizeof(double));
   return FGB_OK;
 }
 
