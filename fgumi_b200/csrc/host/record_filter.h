@@ -53,35 +53,39 @@ FGB_HD size_t fixed_size(uint8_t t) {
   }
 }
 
-// bam_fields::find_tag_position semantics: first occurrence, stops at malformed data.  *entry (optional) = the
-// entry's offset in `a` and *entry_end its end, when found.
+// tag_value_size (fields.rs:289-310) of the entry at a + p, p + 3 <= an: its value's bytes, 0 when its type byte is
+// unknown, a Z / H string lacks its NUL or a B array its header or element type; *sub / *count: a B array's element
+// type and count
+FGB_HD size_t value_size(const uint8_t* a, size_t an, size_t p, uint8_t* sub, uint32_t* count) {
+  const uint8_t vt = a[p + 2];
+  const size_t size = fixed_size(vt);
+  if (size) return size;
+  if (vt == 'Z' || vt == 'H') {
+    size_t z = p + 3;
+    while (z < an && a[z]) ++z;
+    return z == an ? 0 : z - (p + 3) + 1;
+  }
+  if (vt != 'B' || an - (p + 3) < 5) return 0;
+  const size_t es = fixed_size(a[p + 3]);
+  if (!es) return 0;
+  *sub = a[p + 3];
+  *count = ld32(a + p + 4);
+  return 5 + static_cast<size_t>(*count) * es;
+}
+
+// bam_fields::find_tag_position semantics for a value lookup: the first occurrence, absent when the walk meets
+// malformed data first or the entry's value runs past `an`.  *entry (optional) = the entry's offset in `a` and
+// *entry_end its end, when found.
 FGB_HD TagRef find_tag(const uint8_t* a, size_t an, const char tag[2], size_t* entry = nullptr,
                        size_t* entry_end = nullptr) {
   TagRef r;
   size_t p = 0;
   while (p + 3 <= an) {
     const uint8_t vt = a[p + 2];
-    size_t size = fixed_size(vt);
     uint8_t sub = 0;
     uint32_t count = 0;
-    if (!size) {
-      if (vt == 'Z' || vt == 'H') {
-        size_t z = p + 3;
-        while (z < an && a[z]) ++z;
-        if (z == an) return r;
-        size = z - (p + 3) + 1;
-      } else if (vt == 'B') {
-        if (an - (p + 3) < 5) return r;
-        sub = a[p + 3];
-        const size_t es = fixed_size(sub);
-        if (!es) return r;
-        count = ld32(a + p + 4);
-        size = 5 + static_cast<size_t>(count) * es;
-      } else {
-        return r;
-      }
-    }
-    if (p + 3 + size > an) return r;
+    const size_t size = value_size(a, an, p, &sub, &count);
+    if (!size || p + 3 + size > an) return r;
     if (a[p] == static_cast<uint8_t>(tag[0]) && a[p + 1] == static_cast<uint8_t>(tag[1])) {
       r.type = vt; r.sub = sub; r.count = vt == 'B' ? count : static_cast<uint32_t>(size);
       r.data = a + p + 3 + (vt == 'B' ? 5 : 0);
@@ -167,10 +171,25 @@ FGB_HD int filter_duplex_read(const uint8_t* aux, size_t an, const Tier& cc, con
   return FGB_FILTER_PASS;
 }
 
-// is_duplex_consensus (filter.rs:443-446): an aD or bD entry of any type
-FGB_HD bool is_duplex(const uint8_t* aux, size_t an) {
-  return find_tag(aux, an, "aD").type || find_tag(aux, an, "bD").type;
+// find_tag_type semantics (tags.rs:56-59 over find_tag_position, :13-34): an entry's name is matched before its value
+// is sized, so the first entry named `tag` counts even when its type byte is unknown or its value runs past the aux
+// data; the walk stops at the first malformed entry before it.  find_tag, which every value lookup goes through,
+// reports such an entry as absent.
+FGB_HD bool has_tag(const uint8_t* a, size_t an, const char tag[2]) {
+  size_t p = 0;
+  while (p + 3 <= an) {
+    if (a[p] == static_cast<uint8_t>(tag[0]) && a[p + 1] == static_cast<uint8_t>(tag[1])) return true;
+    uint8_t sub;
+    uint32_t count;
+    const size_t size = value_size(a, an, p, &sub, &count);
+    if (!size) return false;
+    p += 3 + size;
+  }
+  return false;
 }
+
+// is_duplex_consensus (filter.rs:443-446): an aD or bD entry, found as find_tag_type finds it
+FGB_HD bool is_duplex(const uint8_t* aux, size_t an) { return has_tag(aux, an, "aD") || has_tag(aux, an, "bD"); }
 
 FGB_HD uint8_t base_code(const uint8_t* rec, size_t so, size_t i) {   // the 4-bit code of base i
   const uint8_t b = rec[so + i / 2];

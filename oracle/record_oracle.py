@@ -1501,7 +1501,11 @@ class OverlappingOracle:
 # Consensus filter (crates/fgumi-consensus/src/filter.rs + src/lib/commands/filter.rs), simplex reads
 # =================================================================================================
 def _aux_tags(aux: bytes):
-    """Walk BAM aux data -> {tag: (type, value)}; B arrays -> (subtype, [values])."""
+    """Walk BAM aux data -> {tag: (type, value)}; B arrays -> (subtype, [values]).  As the reference's lookups
+    (find_tag_position, raw-bam tags.rs:13-34) read it: a repeated tag is its first entry, and the walk ends at the
+    first entry whose type byte is unknown, whose Z / H string lacks its NUL, whose B array has an unknown element
+    type or whose value runs past the data (tag_value_size, fields.rs:289-310; the value lookups refuse a value cut
+    short)."""
     out, p = {}, 0
     fixed = {"A": ("<c", 1), "c": ("<b", 1), "C": ("<B", 1), "s": ("<h", 2), "S": ("<H", 2),
              "i": ("<i", 4), "I": ("<I", 4), "f": ("<f", 4)}
@@ -1510,21 +1514,52 @@ def _aux_tags(aux: bytes):
         p += 3
         if vt in fixed:
             fmt, n = fixed[vt]
-            out[tag] = (vt, struct.unpack_from(fmt, aux, p)[0])
+            if p + n > len(aux):
+                break
+            val = (vt, struct.unpack_from(fmt, aux, p)[0])
             p += n
         elif vt in "ZH":
-            e = aux.index(b"\0", p)
-            out[tag] = (vt, bytes(aux[p:e]))
+            e = aux.find(b"\0", p)
+            if e < 0:
+                break
+            val = (vt, bytes(aux[p:e]))
             p = e + 1
         elif vt == "B":
+            if p + 5 > len(aux) or chr(aux[p]) not in fixed:
+                break
             st = chr(aux[p])
             (cnt,) = struct.unpack_from("<I", aux, p + 1)
             fmt, n = fixed[st]
-            out[tag] = ("B" + st, list(struct.unpack_from("<%d%s" % (cnt, fmt[1]), aux, p + 5)))
+            if p + 5 + cnt * n > len(aux):
+                break
+            val = ("B" + st, list(struct.unpack_from("<%d%s" % (cnt, fmt[1]), aux, p + 5)))
             p += 5 + cnt * n
         else:
             break
+        out.setdefault(tag, val)
     return out
+
+
+def _has_tag(aux: bytes, tag: bytes) -> bool:
+    """find_tag_type (raw-bam tags.rs:56-59): find_tag_position matches an entry's name before it sizes the value, so
+    the first entry named `tag` counts even when its type byte is unknown or its value runs past the data; the walk
+    ends at a malformed entry before it."""
+    fixed = {"A": 1, "c": 1, "C": 1, "s": 2, "S": 2, "i": 4, "I": 4, "f": 4}
+    p = 0
+    while p + 3 <= len(aux):
+        if bytes(aux[p:p + 2]) == tag:
+            return True
+        vt = chr(aux[p + 2])
+        size = fixed.get(vt)
+        if vt in "ZH":
+            e = aux.find(b"\0", p + 3)
+            size = None if e < 0 else e - (p + 3) + 1
+        elif vt == "B" and p + 8 <= len(aux) and chr(aux[p + 3]) in fixed:
+            size = 5 + struct.unpack_from("<I", aux, p + 4)[0] * fixed[chr(aux[p + 3])]
+        if size is None:
+            return False
+        p += 3 + size
+    return False
 
 
 @dataclass
@@ -1650,8 +1685,7 @@ class SimplexFilterOracle:
 
 # ---- duplex consensus reads (filter.rs:443-447, 477-557, 621-639, 702-806) ----------------------
 def is_duplex_consensus(aux: bytes) -> bool:                        # filter.rs:443-446
-    tags = _aux_tags(aux)
-    return b"aD" in tags or b"bD" in tags
+    return _has_tag(aux, b"aD") or _has_tag(aux, b"bD")
 
 
 def _find_int(tags, tag):                                           # bam_fields::find_int_tag: any integer type

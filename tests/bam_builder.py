@@ -4,6 +4,7 @@ import struct
 
 SEQ_CODE = {c: i for i, c in enumerate(b"=ACMGRSVTWYHKDBN")}
 CIGAR_OPS = "MIDNSHP=X"
+B_FORMATS = {"Bc": "b", "BC": "B", "Bs": "h", "BS": "H", "Bi": "i", "BI": "I", "Bf": "f"}
 
 
 def encode_op(op: int, length: int) -> int:
@@ -23,7 +24,9 @@ def cigar_from_string(s: str):
 
 def make_record(name=b"r", flags=0, ref_id=0, pos=0, mapq=60, cigar=None, mate_ref_id=-1, mate_pos=-1,
                 tlen=0, seq=b"", quals=None, tags=()):
-    """tags: sequence of (b"XX", "Z"|"i"|"f"|..., value)"""
+    """tags: sequence of (b"XX", type, value): "A" (one byte), "Z" / "H" (bytes), "c" "C" "s" "S" "i" "I" "f" (a
+    number), "Bc" "BC" "Bs" "BS" "Bi" "BI" "Bf" (a list of numbers), or "raw": the tag, then `value`'s bytes as they
+    are -- the type byte and value of an entry that may be malformed or cut short."""
     cigar = cigar if cigar is not None else ([encode_op(0, len(seq))] if len(seq) else [])
     if isinstance(cigar, str):
         cigar = cigar_from_string(cigar)
@@ -42,8 +45,12 @@ def make_record(name=b"r", flags=0, ref_id=0, pos=0, mapq=60, cigar=None, mate_r
     rec += quals
     for tag, typ, val in tags:
         rec += tag
-        if typ == "Z":
-            rec += b"Z" + bytes(val) + b"\0"
+        if typ in ("Z", "H"):
+            rec += typ.encode() + bytes(val) + b"\0"
+        elif typ == "A":
+            rec += b"A" + bytes(val)[:1]
+        elif typ == "raw":
+            rec += bytes(val)
         elif typ == "i":
             rec += b"i" + struct.pack("<i", val)
         elif typ == "C":
@@ -52,10 +59,8 @@ def make_record(name=b"r", flags=0, ref_id=0, pos=0, mapq=60, cigar=None, mate_r
             rec += typ.encode() + struct.pack({"c": "<b", "s": "<h", "S": "<H", "I": "<I"}[typ], val)
         elif typ == "f":
             rec += b"f" + struct.pack("<f", val)
-        elif typ == "Bs":
-            rec += b"Bs" + struct.pack("<I", len(val)) + struct.pack("<%dh" % len(val), *val)
-        elif typ == "BC":
-            rec += b"BC" + struct.pack("<I", len(val)) + bytes(val)
+        elif typ in B_FORMATS:
+            rec += typ.encode() + struct.pack("<I", len(val)) + struct.pack("<%d%s" % (len(val), B_FORMATS[typ]), *val)
         else:
             raise ValueError(typ)
     return bytes(rec)

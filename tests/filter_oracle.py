@@ -269,7 +269,7 @@ def process_record(r: bytearray, idx: int, cfg: Config, sq, genome) -> Tuple[int
     if cfg.reverse_per_base_tags:
         reverse_per_base_tags(r)
     cc, ab, ba = cfg.tiers()
-    duplex = find_tag(bytes(r), b"aD") is not None or find_tag(bytes(r), b"bD") is not None
+    duplex = R.is_duplex_consensus(bytes(r[aux_offset(bytes(r)):]))
     if duplex:
         masked = R.mask_duplex_bases(r, cc, ab, ba, cfg.min_base_quality, cfg.require_ss_agreement)
     else:

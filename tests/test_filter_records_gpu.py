@@ -191,6 +191,7 @@ def _err_cases(contigs):
         ("truncated", mapped(ref_id=0, pos=10)[:-4], True),
         ("shorter than 32 bytes", b"\0" * 20, True),
         ("two primary R1s", None, True),
+        ("one base past the contig's end", mapped(ref_id=0, pos=len(contigs[0][1]) - 9), True),
     ]
 
 
@@ -219,7 +220,7 @@ def test_first_of_two_errors(mods, world, later):
         rf.close()
 
 
-@pytest.mark.parametrize("k", range(9))
+@pytest.mark.parametrize("k", range(10))
 def test_errors_fail_the_call(mods, world, k):
     F, _ = mods
     contigs, ref, genome = world
