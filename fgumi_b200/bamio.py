@@ -381,3 +381,50 @@ def filter_file(in_path: str, out_path: str, record_filter, reference=None, reje
     tm.update({"filter_s": t_filter, "input_records": float(len(rec_off) - 1), "output_bytes": float(out_bytes)})
     tm.update({k: float(v) for k, v in counts.items()})
     return tm
+
+
+_METRICS_SUFFIX = {"family_sizes": ".family_sizes.txt", "duplex_family_sizes": ".duplex_family_sizes.txt",
+                   "umi_counts": ".umi_counts.txt", "duplex_umi_counts": ".duplex_umi_counts.txt"}
+
+
+def _metrics_file(in_path: str, prefix: str, duplex: bool, intervals: str, n_threads: int, batch_records: int,
+                  device: int, **opts) -> Dict[str, float]:
+    from .metrics import MetricsCollector
+    text, bodies, rec_off, tm = read_bam(in_path, n_threads)
+    iv = None
+    if intervals is not None:
+        with open(intervals, "rb") as f:
+            iv = f.read()
+    m = MetricsCollector(text, duplex=duplex, intervals=iv, device=device, n_threads=n_threads, **opts)
+    t0 = time.perf_counter()
+    try:
+        for b, e in qname_batches(bodies, rec_off, batch_records):   # bad_record counts over every call already
+            m.add_records(bodies[int(rec_off[b]):int(rec_off[e])], rec_off[b:e + 1] - rec_off[b])
+        tables = m.finish()
+        tm["metrics_s"] = time.perf_counter() - t0
+        tm.update({k: float(v) for k, v in m.stats().items()})
+    finally:
+        m.close()
+    suffix = dict(_METRICS_SUFFIX, yield_metrics=".duplex_yield_metrics.txt" if duplex else ".simplex_yield_metrics.txt")
+    for name, body in tables.items():
+        with open(prefix + suffix[name], "w") as f:
+            f.write(body)
+    return tm
+
+
+def duplex_metrics_file(in_path: str, prefix: str, intervals: str = None, min_ab_reads: int = 1, min_ba_reads: int = 1,
+                        duplex_umi_counts: bool = False, n_threads: int = 4, batch_records: int = 1_000_000,
+                        device: int = 0) -> Dict[str, float]:
+    """`fgumi duplex-metrics -i in.bam -o prefix [-l intervals] [--min-ab-reads] [--min-ba-reads]
+    [--duplex-umi-counts]`: writes <prefix>.family_sizes.txt, .duplex_family_sizes.txt, .duplex_yield_metrics.txt,
+    .umi_counts.txt and, with duplex_umi_counts, .duplex_umi_counts.txt.  The input is read into memory whole and fed
+    in batches cut at QNAME changes; a failure raises metrics.MetricsError naming the record in the whole input."""
+    return _metrics_file(in_path, prefix, True, intervals, n_threads, batch_records, device,
+                         min_ab_reads=min_ab_reads, min_ba_reads=min_ba_reads, duplex_umi_counts=duplex_umi_counts)
+
+
+def simplex_metrics_file(in_path: str, prefix: str, intervals: str = None, min_reads: int = 1, n_threads: int = 4,
+                         batch_records: int = 1_000_000, device: int = 0) -> Dict[str, float]:
+    """`fgumi simplex-metrics -i in.bam -o prefix [-l intervals] [--min-reads]`: writes <prefix>.family_sizes.txt,
+    .simplex_yield_metrics.txt and .umi_counts.txt, as duplex_metrics_file does."""
+    return _metrics_file(in_path, prefix, False, intervals, n_threads, batch_records, device, min_reads=min_reads)

@@ -2714,6 +2714,8 @@ uint32_t fgb_struct_size(uint32_t id) {
     case 12: return sizeof(fgb_sort_options);
     case 13: return sizeof(fgb_dedup_options);
     case 14: return sizeof(fgb_record_filter_options);
+    case 15: return sizeof(fgb_metrics_options);
+    case 16: return sizeof(fgb_metrics_template);
     default: return 0;
   }
 }

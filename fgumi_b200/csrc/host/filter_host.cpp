@@ -69,30 +69,6 @@ bool parse_fasta(const uint8_t* f, size_t n, fgb_reference* r, std::vector<uint8
   return true;
 }
 
-// The @SQ SN names of the header, in order
-std::vector<std::string> sq_names(std::string_view text) {
-  std::vector<std::string> out;
-  size_t p = 0;
-  while (p < text.size()) {
-    size_t e = text.find('\n', p);
-    if (e == std::string_view::npos) e = text.size();
-    const std::string_view ln = text.substr(p, e - p);
-    if (ln.substr(0, 4) == "@SQ\t") {
-      std::string sn;
-      for (size_t q = 4; q <= ln.size();) {
-        size_t t = ln.find('\t', q);
-        if (t == std::string_view::npos) t = ln.size();
-        if (ln.substr(q, 3) == "SN:") { sn = std::string(ln.substr(q + 3, t - q - 3)); break; }
-        q = t + 1;
-      }
-      if (!sn.empty() && sn.back() == '\r') sn.pop_back();
-      out.push_back(sn);
-    }
-    p = e + 1;
-  }
-  return out;
-}
-
 // The checks that need only a record's fixed fields (regenerate_alignment_tags_raw's, alignment_tags.rs:259-291, and
 // the command's no-reference check, commands/filter.rs:758-768): "" or why record i fails the call; *layout: the
 // record is cut short.
@@ -119,7 +95,7 @@ fgb_status filter_impl(const link::HandleInfo& hi, const fgb_record_filter_optio
   double* tm = hi.timing;
   auto t_host = std::chrono::steady_clock::now();
   // header-level checks: the first failing record in input order
-  const std::vector<std::string> sq = sq_names(header);
+  const std::vector<std::string> sq = link::sq_names(header);
   uint64_t hb = n;
   std::string herr;
   fgb_status hst = FGB_OK;

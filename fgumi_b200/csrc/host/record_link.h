@@ -1,4 +1,4 @@
-// The host-device plumbing of the record commands' drivers (sort_host.cpp, filter_host.cpp): the handle as a driver
+// The host-device plumbing of the record commands' drivers (sort_host.cpp, filter_host.cpp, metrics_host.cpp): the handle as a driver
 // sees it, the device budget, failure texts, and one call's resources -- its device buffers, the two page-locked
 // staging buffers through which each run's bytes cross the link, and its timing events.
 #pragma once
@@ -10,6 +10,7 @@
 #include <cstring>
 #include <new>
 #include <string>
+#include <string_view>
 #include <vector>
 
 #include "../../../include/fgumi_b200.h"
@@ -37,6 +38,30 @@ HandleInfo info(fgb_handle* h, Command c);   // defined in capi.cu, which owns t
 
 inline double ms_since(std::chrono::steady_clock::time_point t) {
   return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
+}
+
+// The @SQ SN names of the header, in order
+inline std::vector<std::string> sq_names(std::string_view text) {
+  std::vector<std::string> out;
+  size_t p = 0;
+  while (p < text.size()) {
+    size_t e = text.find('\n', p);
+    if (e == std::string_view::npos) e = text.size();
+    const std::string_view ln = text.substr(p, e - p);
+    if (ln.substr(0, 4) == "@SQ\t") {
+      std::string sn;
+      for (size_t q = 4; q <= ln.size();) {
+        size_t t = ln.find('\t', q);
+        if (t == std::string_view::npos) t = ln.size();
+        if (ln.substr(q, 3) == "SN:") { sn = std::string(ln.substr(q + 3, t - q - 3)); break; }
+        q = t + 1;
+      }
+      if (!sn.empty() && sn.back() == '\r') sn.pop_back();
+      out.push_back(sn);
+    }
+    p = e + 1;
+  }
+  return out;
 }
 
 // memcpy on n_threads host threads (the staging copies are what bounds the upload and download)

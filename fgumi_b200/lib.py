@@ -241,6 +241,24 @@ class FgbRecordFilterOptions(C.Structure):
 FILTER_STAT_NAMES = ("total", "passed", "failed", "bases_masked")
 
 
+class FgbMetricsOptions(C.Structure):
+    _fields_ = [("mode", C.c_uint32), ("n_threads", C.c_uint32), ("min_ab_reads", C.c_uint64),
+                ("min_ba_reads", C.c_uint64), ("min_reads", C.c_uint64), ("duplex_umi_counts", C.c_uint8),
+                ("reserved", C.c_uint8 * 7), ("device_bytes", C.c_uint64)]
+
+
+class FgbMetricsTemplate(C.Structure):
+    _fields_ = [("ref1", C.c_int32), ("start1", C.c_int32), ("ref2", C.c_int32), ("start2", C.c_int32),
+                ("strand1", C.c_uint8), ("strand2", C.c_uint8), ("status", C.c_uint8), ("bucket", C.c_uint8),
+                ("contig", C.c_int32), ("ins_start", C.c_int32), ("ins_end", C.c_int32), ("mi_kind", C.c_uint8),
+                ("mi_canonical", C.c_uint8), ("name_ascii", C.c_uint8), ("reserved", C.c_uint8), ("r1", C.c_uint32),
+                ("mi_base", C.c_uint64), ("mi_off", C.c_uint32), ("mi_len", C.c_uint32), ("rx_off", C.c_uint32),
+                ("rx_len", C.c_uint32)]
+
+
+METRICS_STAT_NAMES = ("records", "templates", "kept", "outside", "groups", "ds_families", "overflow", "runs")
+
+
 class FgbUmiKey(C.Structure):
     _fields_ = [("bits", C.c_uint64), ("str_off", C.c_uint64), ("str_len", C.c_uint32), ("count", C.c_uint32),
                 ("first", C.c_uint32), ("dash", C.c_uint32), ("len", C.c_uint8), ("flags", C.c_uint8),
@@ -283,6 +301,10 @@ SYMBOLS = (
     "fgb_deduper_stats", "fgb_deduper_histogram", "fgb_deduper_last_timing", "fgb_record_quality_scores",
     "fgb_reference_create", "fgb_reference_destroy", "fgb_reference_contigs", "fgb_reference_contig",
     "fgb_filter_records", "fgb_filter_last_timing",
+    "fgb_host_metrics_templates", "fgb_host_metrics_name_fraction", "fgb_host_metrics_bucket",
+    "fgb_host_metrics_intervals", "fgb_host_metrics_format_float", "fgb_metrics_create", "fgb_metrics_destroy",
+    "fgb_metrics_last_error", "fgb_metrics_add_records", "fgb_metrics_finish", "fgb_metrics_table",
+    "fgb_metrics_stats", "fgb_metrics_last_timing",
 )
 
 _lib = None
@@ -541,6 +563,35 @@ def load() -> C.CDLL:
     lib.fgb_filter_records.restype = C.c_int32
     lib.fgb_filter_last_timing.argtypes = [vp, vp]
     lib.fgb_filter_last_timing.restype = C.c_int32
+    lib.fgb_host_metrics_templates.argtypes = [C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t, vp, vp, u64, vp, u64,
+                                               C.POINTER(u64), C.POINTER(u64)]
+    lib.fgb_host_metrics_templates.restype = C.c_int32
+    lib.fgb_host_metrics_name_fraction.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(C.c_int32),
+                                                   C.POINTER(C.c_double), C.POINTER(u32)]
+    lib.fgb_host_metrics_name_fraction.restype = C.c_int32
+    lib.fgb_host_metrics_bucket.argtypes = [C.c_int32]
+    lib.fgb_host_metrics_bucket.restype = u32
+    lib.fgb_host_metrics_intervals.argtypes = [C.c_char_p, C.c_size_t, vp, vp, vp, vp, u64, C.POINTER(u64)]
+    lib.fgb_host_metrics_intervals.restype = C.c_int32
+    lib.fgb_host_metrics_format_float.argtypes = [C.c_double, C.c_char_p, C.c_size_t]
+    lib.fgb_host_metrics_format_float.restype = C.c_size_t
+    lib.fgb_metrics_create.argtypes = [C.c_int, C.POINTER(FgbMetricsOptions), C.c_char_p, C.c_size_t, C.c_char_p,
+                                       C.c_size_t, C.POINTER(vp)]
+    lib.fgb_metrics_create.restype = C.c_int32
+    lib.fgb_metrics_destroy.argtypes = [vp]
+    lib.fgb_metrics_destroy.restype = None
+    lib.fgb_metrics_last_error.argtypes = [vp, C.c_char_p, C.c_size_t]
+    lib.fgb_metrics_last_error.restype = C.c_size_t
+    lib.fgb_metrics_add_records.argtypes = [vp, vp, vp, u64, C.POINTER(u64)]
+    lib.fgb_metrics_add_records.restype = C.c_int32
+    lib.fgb_metrics_finish.argtypes = [vp, C.POINTER(u64)]
+    lib.fgb_metrics_finish.restype = C.c_int32
+    lib.fgb_metrics_table.argtypes = [vp, u32, C.POINTER(C.c_char_p), C.POINTER(u64)]
+    lib.fgb_metrics_table.restype = C.c_int32
+    lib.fgb_metrics_stats.argtypes = [vp, vp]
+    lib.fgb_metrics_stats.restype = C.c_int32
+    lib.fgb_metrics_last_timing.argtypes = [vp, vp]
+    lib.fgb_metrics_last_timing.restype = C.c_int32
     lib.fgb_struct_size.argtypes = [C.c_uint32]
     lib.fgb_struct_size.restype = C.c_uint32
     _lib = lib

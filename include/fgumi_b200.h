@@ -1177,11 +1177,111 @@ fgb_status fgb_filter_records(fgb_handle* h, const fgb_record_filter_options* op
  * the environment variable FGB_FILTER_STAGE_BYTES (at least 4096) lowers that, read on every call. */
 fgb_status fgb_filter_last_timing(const fgb_handle* h, double ms[6]);
 
+/* ---- `fgumi duplex-metrics` / `fgumi simplex-metrics` on raw records (src/lib/commands/{shared_metrics,
+ * duplex_metrics,simplex_metrics}.rs, crates/fgumi-metrics): the QC tables of a UMI-grouped stream (group's output).
+ * Per template (consecutive QNAME run of at least two records, Template::from_records order): R1 / R2 = the first
+ * record that is paired, mapped with its mate mapped, of that segment, neither secondary nor supplementary (both are
+ * required); R1's MI and RX must be Z strings in UTF-8 (else the call fails, before the interval test); the
+ * ReadInfoKey (ref, unclipped 5', strand) of both reads, the earlier first, groups consecutive templates into
+ * coordinate groups; the insert span (R1's own range when the mates are on different contigs) is tested against the
+ * intervals; the read name's htsjdk Murmur3 (seed 42, UTF-16 code units) gives the template's downsampling fraction.
+ * The template pass and the family counting (CS / SS / DS sizes, (ab, ba) pairs, per fraction) run on the device; the
+ * UMI consensus of the 100 % fraction and the tables run on host threads. */
+enum { FGB_METRICS_SIMPLEX = 0, FGB_METRICS_DUPLEX = 1 };
+typedef struct fgb_metrics_options {
+  uint32_t mode;              /* FGB_METRICS_SIMPLEX / FGB_METRICS_DUPLEX                                         */
+  uint32_t n_threads;         /* host threads (templates, UMI consensus); 0 or 1 = the calling thread             */
+  uint64_t min_ab_reads;      /* duplex: --min-ab-reads (1); must be >= min_ba_reads                              */
+  uint64_t min_ba_reads;      /* duplex: --min-ba-reads (1)                                                       */
+  uint64_t min_reads;         /* simplex: --min-reads (1)                                                         */
+  uint8_t duplex_umi_counts;  /* duplex: --duplex-umi-counts                                                      */
+  uint8_t reserved[7];
+  uint64_t device_bytes;      /* device-memory budget of one staged run; 0 = from cudaMemGetInfo                 */
+} fgb_metrics_options;
+/* The template statuses of fgb_host_metrics_templates. */
+enum {
+  FGB_MT_SKIP = 0,            /* fewer than 2 records, no R1 or R2, or a read without a CIGAR                     */
+  FGB_MT_OUTSIDE = 1,         /* outside every interval                                                           */
+  FGB_MT_KEPT = 2,
+  FGB_MT_ERR_MI_MISSING = 3, FGB_MT_ERR_MI_UTF8 = 4, FGB_MT_ERR_RX_MISSING = 5, FGB_MT_ERR_RX_UTF8 = 6
+};
+typedef struct fgb_metrics_template {   /* one template as the device's template pass sees it                     */
+  int32_t ref1, start1, ref2, start2;   /* ReadInfoKey: the earlier (ref, unclipped 5', 0-based) read first        */
+  uint8_t strand1, strand2;             /* reverse strand                                                          */
+  uint8_t status;                       /* FGB_MT_*                                                                */
+  uint8_t bucket;                       /* the first fraction index i with hash_fraction <= 0.05 (i + 1)           */
+  int32_t contig;                       /* R1's ref_id                                                             */
+  int32_t ins_start, ins_end;           /* 1-based insert span                                                     */
+  uint8_t mi_kind;                      /* 0: no suffix, 1: "/A", 2: "/B"                                          */
+  uint8_t mi_canonical;                 /* the MI's base is a canonical decimal: mi_base is its value              */
+  uint8_t name_ascii;                   /* 0: the name has a byte >= 0x80 and its bucket comes from the host       */
+  uint8_t reserved;
+  uint32_t r1;                          /* R1's record index (in the call)                                         */
+  uint64_t mi_base;
+  uint32_t mi_off, mi_len, rx_off, rx_len;   /* the MI / RX strings, offsets within R1's record                    */
+} fgb_metrics_template;
+/* The template pass on host threads, the same code as the device's: templates = the QNAME runs of the records
+ * (record i = records[rec_off[i] .. rec_off[i+1]), no block_size prefix), out[t] for run t (cap >= runs), *n_templates.
+ * `intervals` (BED or Picard interval list text, NULL = none) are matched by contig name against `header_text`'s @SQ
+ * lines.  A malformed record gives FGB_ERR_LAYOUT, a template with two primary R1s or R2s FGB_ERR_INVALID_ARG, each
+ * with *bad_record; an unparsable interval line FGB_ERR_INVALID_ARG. */
+fgb_status fgb_host_metrics_templates(const char* header_text, size_t header_len, const char* intervals,
+                                      size_t intervals_len, const uint8_t* records, const uint64_t* rec_off,
+                                      uint64_t n_records, fgb_metrics_template* out, uint64_t cap,
+                                      uint64_t* n_templates, uint64_t* bad_record);
+/* compute_hash_fraction (shared_metrics.rs:106-184): the name (`len` bytes, lossy UTF-8 to UTF-16) -> the Murmur3 hash,
+ * wrapping_abs(hash) / i32::MAX and the bucket (0..19). */
+fgb_status fgb_host_metrics_name_fraction(const uint8_t* name, size_t len, int32_t* hash, double* fraction,
+                                          uint32_t* bucket);
+/* The bucket of a Murmur3 hash, as the device computes it. */
+uint32_t fgb_host_metrics_bucket(int32_t hash);
+/* BED or Picard interval list text (parse_intervals, shared_metrics.rs:186-253) -> 0-based half-open intervals:
+ * *n entries of (name offset, name length, start, end) into `text`, written when cap >= *n. */
+fgb_status fgb_host_metrics_intervals(const char* text, size_t len, uint64_t* name_off, uint64_t* name_len,
+                                      int64_t* start, int64_t* end, uint64_t cap, uint64_t* n);
+/* The TSV float text (csv 1.1 / ryu 1.0 shortest round trip, DESIGN.md section 13) of v; returns its length. */
+size_t fgb_host_metrics_format_float(double v, char* buf, size_t cap);
+
+typedef struct fgb_metrics fgb_metrics;
+/* min_ab_reads < min_ba_reads, an unknown mode or unparsable intervals give FGB_ERR_INVALID_ARG.  device ==
+ * FGB_DEVICE_NONE: a planning-only collector -- add_records and finish fail with FGB_ERR_NO_DEVICE. */
+fgb_status fgb_metrics_create(int device, const fgb_metrics_options* opt, const char* header_text, size_t header_len,
+                              const char* intervals, size_t intervals_len, fgb_metrics** out);
+void fgb_metrics_destroy(fgb_metrics* m);
+size_t fgb_metrics_last_error(const fgb_metrics* m, char* buf, size_t buf_len);
+/* Streams records (a call holds whole QNAME runs; coordinate groups may continue into the next call).  The first
+ * paired, primary R1 of the stream with aD and bD, or cD, fails the call (a consensus input).  Errors fail the call
+ * with *bad_record = the record index (counted over every call) of the first bad template's first record, or of a
+ * failing UMI family's first template, and poison the collector. */
+fgb_status fgb_metrics_add_records(fgb_metrics* m, const uint8_t* records, const uint64_t* rec_off, uint64_t n_records,
+                                   uint64_t* bad_record);
+/* Closes the last coordinate group and builds the tables; no records may follow. */
+fgb_status fgb_metrics_finish(fgb_metrics* m, uint64_t* bad_record);
+enum {   /* the tables of fgb_metrics_table, each one output file */
+  FGB_MTABLE_FAMILY_SIZES = 0,        /* <prefix>.family_sizes.txt                                    */
+  FGB_MTABLE_DUPLEX_FAMILY_SIZES = 1, /* <prefix>.duplex_family_sizes.txt (duplex)                    */
+  FGB_MTABLE_YIELD = 2,               /* <prefix>.duplex_yield_metrics.txt / .simplex_yield_metrics.txt */
+  FGB_MTABLE_UMI_COUNTS = 3,          /* <prefix>.umi_counts.txt                                      */
+  FGB_MTABLE_DUPLEX_UMI_COUNTS = 4    /* <prefix>.duplex_umi_counts.txt (duplex with duplex_umi_counts) */
+};
+/* A finished collector's table `which` as TSV text (valid until destroy); FGB_ERR_INVALID_ARG for a table the mode
+ * does not write. */
+fgb_status fgb_metrics_table(const fgb_metrics* m, uint32_t which, const char** text, uint64_t* len);
+enum {
+  FGB_MSTAT_RECORDS = 0, FGB_MSTAT_TEMPLATES = 1, FGB_MSTAT_KEPT = 2, FGB_MSTAT_OUTSIDE = 3, FGB_MSTAT_GROUPS = 4,
+  FGB_MSTAT_DS_FAMILIES = 5, FGB_MSTAT_OVERFLOW = 6, FGB_MSTAT_RUNS = 7, FGB_METRICS_NSTATS = 8
+};
+fgb_status fgb_metrics_stats(const fgb_metrics* m, uint64_t stats[FGB_METRICS_NSTATS]);
+/* Where the collector has spent its time so far, in ms: [0] template pass (upload, kernel, download), [1] family pass
+ * (upload, group scan, sorts, counting kernels, download), [2] UMI consensus, [3] host assembly (templates, tables).
+ * The staging buffers are at most 64 MiB; FGB_METRICS_STAGE_BYTES (at least 4096) lowers that, read on each call. */
+fgb_status fgb_metrics_last_timing(const fgb_metrics* m, double ms[4]);
+
 /* sizeof() of the ABI structs as this library was compiled, so a binding can check its own layout:
  * 0 fgb_caller_options, 1 fgb_filter_params, 2 fgb_submit_options, 3 fgb_raw_columns,
  * 4 fgb_raw_read, 5 fgb_batch, 6 fgb_codec_params, 7 fgb_params, 8 fgb_duplex_filter_params,
  * 9 fgb_record_columns, 10 fgb_umi_options, 11 fgb_group_options, 12 fgb_sort_options, 13 fgb_dedup_options,
- * 14 fgb_record_filter_options; 0 for an unknown id. */
+ * 14 fgb_record_filter_options, 15 fgb_metrics_options, 16 fgb_metrics_template; 0 for an unknown id. */
 uint32_t fgb_struct_size(uint32_t id);
 
 #ifdef __cplusplus
