@@ -244,21 +244,25 @@ std::vector<std::string> split_dash(std::string_view s) {
   }
 }
 
-// P(A <= x), A ~ Binomial(n, 0.5)
-double binom_cdf_half(uint64_t x, uint64_t n) {
-  if (x >= n) return 1.0;
-  const double ln2 = std::log(2.0), lgn = std::lgamma(static_cast<double>(n) + 1);
-  auto pmf = [&](uint64_t k) {
-    return std::exp(lgn - std::lgamma(static_cast<double>(k) + 1) - std::lgamma(static_cast<double>(n - k) + 1) -
-                    static_cast<double>(n) * ln2);
-  };
-  double s = 0;
-  if (2 * x <= n) {
-    for (uint64_t k = 0; k <= x; ++k) s += pmf(k);
-    return s;
+// P(lower <= A <= upper), A ~ Binomial(n, 0.5), lower <= upper <= n: every term relative to the mode's by the ratio
+// pmf(k + 1) / pmf(k) = (n - k) / (k + 1), the interval's terms over all of them.  A term is off by about its distance
+// from the mode in ulps, and no two CDFs near 0.5 are subtracted, so a short interval amid the mass (min-ab and
+// min-ba near n / 2) keeps its relative accuracy; lgamma terms lose ~ n ulps of lgamma(n) at large n.
+double binom_interval_half(uint64_t lower, uint64_t upper, uint64_t n) {
+  const uint64_t m = n / 2;
+  double all = 1.0, in = lower <= m && m <= upper ? 1.0 : 0.0, t = 1.0;
+  for (uint64_t k = m; k < n && t > 0; ++k) {   // t = pmf(k + 1) / pmf(m)
+    t *= static_cast<double>(n - k) / static_cast<double>(k + 1);
+    all += t;
+    if (k + 1 >= lower && k + 1 <= upper) in += t;
   }
-  for (uint64_t k = x + 1; k <= n; ++k) s += pmf(k);
-  return 1.0 - s;
+  t = 1.0;
+  for (uint64_t k = m; k > 0 && t > 0; --k) {   // t = pmf(k - 1) / pmf(m)
+    t *= static_cast<double>(k) / static_cast<double>(n - k + 1);
+    all += t;
+    if (k - 1 >= lower && k - 1 <= upper) in += t;
+  }
+  return in / all;
 }
 
 }  // namespace
@@ -789,8 +793,7 @@ void build_tables(fgb_metrics* m) {
           auto it = prob.find(z);
           if (it == prob.end()) {
             const uint64_t upper = z - min_ba, lower = min_ab;
-            const double p = upper >= lower ? binom_cdf_half(upper, z) - (lower > 0 ? binom_cdf_half(lower - 1, z) : 0.0)
-                                            : 0.0;
+            const double p = upper >= lower ? binom_interval_half(lower, upper, z) : 0.0;
             it = prob.emplace(z, p).first;
           }
           for (uint64_t i = 0; i < c; ++i) ideal += it->second;

@@ -136,9 +136,10 @@ def _utf8(b: bytes) -> Optional[str]:
         return None
 
 
-def templates(header_text: bytes, records: Sequence[bytes], ivs, first_index: int = 0):
+def templates(header_text: bytes, records: Sequence[bytes], ivs, first_index: int = 0, overlap=None):
     """(key, mi, rx, hash fraction, first record index) per kept template, in stream order: a generator, so that an
-    error is raised where the reference's stream meets it."""
+    error is raised where the reference's stream meets it.  overlap(ref_name, start, end), when given, replaces
+    overlaps(ivs, ...) (tests/metrics_shapes.py's index for long interval lists)."""
     sq = [ln.split(b"\tSN:")[1].split(b"\t")[0].decode(errors="replace")
           for ln in header_text.split(b"\n") if ln.startswith(b"@SQ\t") and b"\tSN:" in ln]
     i = 0
@@ -179,7 +180,7 @@ def templates(header_text: bytes, records: Sequence[bytes], ivs, first_index: in
         rev1, rev2 = bool(G.flags(r1) & 0x10), bool(G.flags(r2) & 0x10)
         key = (t1, s1, rev1, t2, s2, rev2) if (t1, s1) <= (t2, s2) else (t2, s2, rev2, t1, s1, rev1)
         ref_name = sq[t1] if t1 < len(sq) else None
-        if not overlaps(ivs, ref_name, start, end):
+        if not (overlap(ref_name, start, end) if overlap is not None else overlaps(ivs, ref_name, start, end)):
             continue
         yield key, mi, rx, hash_fraction(nm), first_index + i0
 
@@ -425,7 +426,7 @@ def umi_rows(d: Dict[str, list]):   # shared.rs:117-135
 
 def collect(header_text: bytes, records: Sequence[bytes], duplex: bool = True, intervals: Optional[bytes] = None,
             min_ab_reads: int = 1, min_ba_reads: int = 1, min_reads: int = 1,
-            duplex_umi_counts: bool = False) -> Dict[str, str]:
+            duplex_umi_counts: bool = False, overlap=None) -> Dict[str, str]:
     if duplex and min_ab_reads < min_ba_reads:
         raise ValueError("--min-ab-reads must be >= --min-ba-reads")
     ci = consensus_input(records)
@@ -435,7 +436,7 @@ def collect(header_text: bytes, records: Sequence[bytes], duplex: bool = True, i
     cols = [Collector(duplex, duplex_umi_counts and f == 1.0) for f in FRACTIONS]
     counts = [0] * len(FRACTIONS)
     group, key = [], None
-    for t in templates(header_text, records, ivs):
+    for t in templates(header_text, records, ivs, overlap=overlap):
         if key != t[0] and group:
             process_group(group, cols, counts, duplex, duplex_umi_counts)
             group = []
@@ -443,6 +444,12 @@ def collect(header_text: bytes, records: Sequence[bytes], duplex: bool = True, i
         key = t[0]
     if group:
         process_group(group, cols, counts, duplex, duplex_umi_counts)
+    return tables(cols, counts, duplex, min_ab_reads, min_ba_reads, min_reads, duplex_umi_counts)
+
+
+def tables(cols: List[Collector], counts: List[int], duplex: bool, min_ab_reads: int = 1, min_ba_reads: int = 1,
+           min_reads: int = 1, duplex_umi_counts: bool = False) -> Dict[str, str]:
+    """The tables of the per-fraction collectors and template counts."""
     main = cols[-1]
     out = {}
     fs_head = ["family_size", "cs_count", "cs_fraction", "cs_fraction_gt_or_eq_size", "ss_count", "ss_fraction",
