@@ -428,3 +428,94 @@ def simplex_metrics_file(in_path: str, prefix: str, intervals: str = None, min_r
     """`fgumi simplex-metrics -i in.bam -o prefix [-l intervals] [--min-reads]`: writes <prefix>.family_sizes.txt,
     .simplex_yield_metrics.txt and .umi_counts.txt, as duplex_metrics_file does."""
     return _metrics_file(in_path, prefix, False, intervals, n_threads, batch_records, device, min_reads=min_reads)
+
+
+def find_dict_path(reference_path: str) -> str:
+    """find_dict_path (reference.rs): ref.dict beside ref.fa, then ref.fa.dict."""
+    import os
+    for p in (os.path.splitext(reference_path)[0] + ".dict", reference_path + ".dict"):
+        if os.path.exists(p):
+            return p
+    raise FileNotFoundError(f"reference dictionary not found for {reference_path}: tried "
+                            f"{os.path.splitext(reference_path)[0]}.dict and {reference_path}.dict")
+
+
+def zipper_header(unmapped_text: bytes, mapped_text: bytes, dict_text: bytes,
+                  command_line: str = "fgumi_b200 zipper") -> bytes:
+    """build_output_header (zipper.rs:210-256), then one @PG chained as group_header chains it: @HD from the unmapped
+    header, @SQ from the sequence dictionary, @RG and @PG from the mapped header first and the unmapped IDs not already
+    present after them and the new @PG last among them, @CO from the unmapped header then the mapped one; lines kept
+    verbatim, in the order HD, SQ, RG, PG, CO."""
+    def lines(text, kind):
+        return [ln for ln in text.decode("utf-8", "replace").split("\n") if ln.startswith(kind)]
+
+    def ident(ln):
+        return next((f[3:] for f in ln.split("\t")[1:] if f.startswith("ID:")), None)
+
+    out = lines(unmapped_text, "@HD")[:1] + lines(dict_text, "@SQ")
+    for kind in ("@RG", "@PG"):
+        kept, seen = [], set()
+        for ln in lines(mapped_text, kind) + lines(unmapped_text, kind):
+            if ident(ln) not in seen:
+                seen.add(ident(ln))
+                kept.append(ln)
+        out += kept
+    # add_pg_record puts the program into the header's program map, which noodles writes before the comments
+    head = group_header(("\n".join(out) + "\n").encode() if out else b"", command_line)
+    comments = lines(unmapped_text, "@CO") + lines(mapped_text, "@CO")
+    return head + ("\n".join(comments) + "\n").encode() if comments else head
+
+
+def _check_sort(text: bytes, what: str) -> None:
+    """check_sort: a header that is not queryname-sorted only warns."""
+    import warnings
+    hd = next((ln for ln in text.decode("utf-8", "replace").split("\n") if ln.startswith("@HD")), "")
+    if "SO:queryname" not in hd.split("\t"):
+        warnings.warn(f"the {what} input does not declare SO:queryname; its templates must still be grouped by name "
+                      "in the same order as the other input")
+
+
+def zipper_file(unmapped_path: str, mapped_path: str, reference_path: str, out_path: str, zipper, n_threads: int = 4,
+                level: int = 1, batch_records: int = 1_000_000,
+                command_line: str = "fgumi_b200 zipper") -> Dict[str, float]:
+    """`fgumi zipper -u unmapped.bam -i mapped.bam -r ref.fa -o out.bam` with an existing zipper.Zipper (its options
+    decide the rest).  The mapped input must be BAM; the sequence dictionary beside the reference gives the @SQ lines.
+    Both inputs are read into memory whole; the unmapped stream is zipped in batches of about batch_records records
+    cut at QNAME changes, each call taking the mapped records the previous calls left, and each batch's output is
+    compressed and written before the next.  A failing batch raises with zipper.bad_record set to the index in the
+    whole unmapped input, or the number of unmapped records plus the index in the whole mapped input."""
+    with open(find_dict_path(reference_path), "rb") as f:
+        dict_text = f.read()
+    ut, ub, uo, tm = read_bam(unmapped_path, n_threads)
+    mt, mb, mo, _ = read_bam(mapped_path, n_threads)
+    _check_sort(ut, "unmapped")
+    _check_sort(mt, "mapped")
+    header = mapped_bam_header(zipper_header(ut, mt, dict_text, command_line))
+    n_u, n_m = len(uo) - 1, len(mo) - 1
+    counts = dict.fromkeys(_l.ZIPPER_STAT_NAMES, 0)
+    t_zip = out_bytes = 0.0
+    m0 = 0
+    batches = list(qname_batches(ub, uo, batch_records)) or [(0, 0)]
+    with open(out_path, "wb") as f:
+        for k, (b, e) in enumerate(batches):
+            t0 = time.perf_counter()
+            try:
+                # offsets are relative to the bodies passed: views, no copy of the remaining mapped offsets
+                data, used, c = zipper.zip(ub, uo[b:e + 1], mb, mo[m0:], last_call=k == len(batches) - 1)
+            except Exception:
+                if zipper.bad_record is not None:
+                    r = zipper.bad_record
+                    zipper.bad_record = b + r if r < e - b else n_u + m0 + (r - (e - b))
+                raise
+            t_zip += time.perf_counter() - t0
+            m0 += used
+            for key in counts:
+                counts[key] += c[key]
+            out_bytes += len(data)
+            _write_bgzf(f, header + data, level, n_threads, False)
+            header = b""
+        _write_bgzf(f, header, level, n_threads)
+    assert m0 == n_m
+    tm.update({"zipper_s": t_zip, "input_records": float(n_u + n_m), "output_bytes": float(out_bytes)})
+    tm.update({key: float(v) for key, v in counts.items()})
+    return tm

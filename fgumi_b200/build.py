@@ -10,7 +10,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libfgumi_b200.so")
 SOURCES = ["capi.cu", "host_tables.cpp", "host/caller_host.cpp", "host/bgzf.cpp", "host/umi_host.cpp",
            "host/group_host.cpp", "host/sort_host.cpp", "host/dedup_host.cpp", "host/filter_host.cpp",
-           "metrics.cu", "host/metrics_host.cpp"]
+           "metrics.cu", "host/metrics_host.cpp", "zipper.cu", "host/zipper_host.cpp"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-maxrregcount=112",      # upper bound only; vote_kernel must land at <= 96 (see _check_vote_kernel)
@@ -118,6 +118,21 @@ def _check_metrics_kernels(ptxas_log: str) -> None:
         raise RuntimeError(f"fgumi_b200 build: ptxas reported {found} metrics kernels, expected 6")
 
 
+def _check_zipper_kernels(ptxas_log: str) -> None:
+    """The zipper's kernels keep a record's plan (mate fields, tag-edit decisions, tc values) in registers: a stack
+    frame or a spill means a source change pushed it into local memory, and fails the build."""
+    import re
+    found = 0
+    for m in re.finditer(r"Function properties for (\S*zipper_(?:sizes|write)_kernel\S*)\n\s*(\d+) bytes stack frame, "
+                         r"(\d+) bytes spill stores", ptxas_log):
+        found += 1
+        if int(m.group(2)) or int(m.group(3)):
+            raise RuntimeError(f"fgumi_b200 build: {m.group(1)} has a {m.group(2)}-byte stack frame and spills "
+                               f"{m.group(3)} bytes (expected none)")
+    if found != 2:
+        raise RuntimeError(f"fgumi_b200 build: ptxas reported {found} zipper kernels, expected 2")
+
+
 def build(force: bool = False, verbose: bool = False) -> str:
     deps = [os.path.join(dp, f) for dp, _, fs in os.walk(CSRC) for f in fs]
     deps.append(os.path.join(HERE, "..", "include", "fgumi_b200.h"))
@@ -136,6 +151,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     _check_score_kernel(r.stdout + r.stderr)
     _check_filter_kernels(r.stdout + r.stderr)
     _check_metrics_kernels(r.stdout + r.stderr)
+    _check_zipper_kernels(r.stdout + r.stderr)
     return OUT
 
 

@@ -133,6 +133,8 @@ struct fgb_handle {
   double sort_timing[6] = {0, 0, 0, 0, 0, 0};        // fgb_sort_last_timing
   double filter_timing[6] = {0, 0, 0, 0, 0, 0};      // fgb_filter_last_timing
   std::vector<uint8_t> filter_kept, filter_rejects;  // fgb_filter_records' output streams
+  double zipper_timing[6] = {0, 0, 0, 0, 0, 0};      // fgb_zipper_last_timing
+  std::vector<uint8_t> zipper_out;                   // fgb_zipper_records' output stream
   struct ScoreBufs {                                 // template scores (dedup_kernels.cuh): own stream, so that they run
     cudaStream_t stream = nullptr;                   // beside fgb_umi_assign; two page-locked chunks alternate
     uint8_t* h_rec[2] = {nullptr, nullptr}; uint64_t* h_off[2] = {nullptr, nullptr};
@@ -1725,6 +1727,9 @@ fgb_status fgb_umi_edges(fgb_handle* h, const fgb_umi_options* opt, const uint8_
 
 // ---- the record commands' view of the handle (host/record_link.h) ------------------------------------------------
 fgb::link::HandleInfo fgb::link::info(fgb_handle* h, Command c) {
+  if (c == Command::kZipper)
+    return HandleInfo{h->device, h->sm_count, h->slots[0].stream, h->submit_pending, &h->last_error,
+                      h->zipper_timing, &h->zipper_out, nullptr};
   const bool filter = c == Command::kFilter;
   return HandleInfo{h->device, h->sm_count, h->slots[0].stream, h->submit_pending, &h->last_error,
                     filter ? h->filter_timing : h->sort_timing, filter ? &h->filter_kept : nullptr,

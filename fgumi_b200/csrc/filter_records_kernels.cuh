@@ -44,15 +44,7 @@ __device__ __forceinline__ uint32_t int_size(int32_t v, uint8_t* type) {
 __device__ __forceinline__ void warp_copy(uint8_t* dst, const uint8_t* src, uint64_t n, int lane) {
   for (uint64_t j = lane; j < n; j += 32) dst[j] = src[j];
 }
-__device__ __forceinline__ uint8_t complement(uint8_t b) {   // reverse_complement_string_tag_in_place
-  switch (b) {
-    case 'A': case 'a': return 'T';
-    case 'T': case 't': return 'A';
-    case 'C': case 'c': return 'G';
-    case 'G': case 'g': return 'C';
-    default: return b;
-  }
-}
+using rfilter::complement;   // reverse_complement_string_tag_in_place
 
 // reverse_per_base_tags_raw (tag_reversal.rs:27-66) on a reverse-strand record's aux area: the B arrays and Z strings
 // cd ce ad ae bd be aq bq reversed element by element, the Z strings ac bc reverse-complemented

@@ -2716,6 +2716,7 @@ uint32_t fgb_struct_size(uint32_t id) {
     case 14: return sizeof(fgb_record_filter_options);
     case 15: return sizeof(fgb_metrics_options);
     case 16: return sizeof(fgb_metrics_template);
+    case 17: return sizeof(fgb_zipper_options);
     default: return 0;
   }
 }

@@ -37,8 +37,20 @@ FGB_HD uint32_t ld32(const uint8_t* p) {
          (static_cast<uint32_t>(p[3]) << 24);
 }
 
+// the complement of reverse_complement_string_tag_in_place (tags.rs:818-836): A / C / G / T in either case to the
+// upper-case complement, any other byte unchanged
+FGB_HD uint8_t complement(uint8_t b) {
+  switch (b) {
+    case 'A': case 'a': return 'T';
+    case 'T': case 't': return 'A';
+    case 'C': case 'c': return 'G';
+    case 'G': case 'g': return 'C';
+    default: return b;
+  }
+}
+
 struct TagRef {
-  uint8_t type = 0;        // 0 = absent; 'B' arrays carry `sub` and `count`
+  uint8_t type = 0;       // 0 = absent; 'B' arrays carry `sub` and `count`
   uint8_t sub = 0;
   uint32_t count = 0;
   const uint8_t* data = nullptr;

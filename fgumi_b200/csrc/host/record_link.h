@@ -33,7 +33,7 @@ struct HandleInfo {
   std::vector<uint8_t>* kept;      // the filter's library-owned output streams (null for the sort)
   std::vector<uint8_t>* rejects;
 };
-enum class Command { kSort, kFilter };
+enum class Command { kSort, kFilter, kZipper };   // kZipper: its output stream is `kept`, `rejects` is null
 HandleInfo info(fgb_handle* h, Command c);   // defined in capi.cu, which owns the handle
 
 inline double ms_since(std::chrono::steady_clock::time_point t) {

@@ -241,6 +241,17 @@ class FgbRecordFilterOptions(C.Structure):
 FILTER_STAT_NAMES = ("total", "passed", "failed", "bases_masked")
 
 
+class FgbZipperOptions(C.Structure):
+    _fields_ = [("exclude_missing_reads", C.c_uint8), ("skip_pa_tags", C.c_uint8),
+                ("restore_unconverted_bases", C.c_uint8), ("reserved", C.c_uint8 * 1), ("n_threads", C.c_uint32),
+                ("device_bytes", C.c_uint64), ("n_remove", C.c_uint64), ("n_reverse", C.c_uint64),
+                ("n_revcomp", C.c_uint64), ("tags_to_remove", C.c_void_p), ("tags_to_reverse", C.c_void_p),
+                ("tags_to_revcomp", C.c_void_p)]
+
+
+ZIPPER_STAT_NAMES = ("merged", "unmapped_only", "excluded", "records_out")
+
+
 class FgbMetricsOptions(C.Structure):
     _fields_ = [("mode", C.c_uint32), ("n_threads", C.c_uint32), ("min_ab_reads", C.c_uint64),
                 ("min_ba_reads", C.c_uint64), ("min_reads", C.c_uint64), ("duplex_umi_counts", C.c_uint8),
@@ -305,6 +316,7 @@ SYMBOLS = (
     "fgb_host_metrics_intervals", "fgb_host_metrics_format_float", "fgb_metrics_create", "fgb_metrics_destroy",
     "fgb_metrics_last_error", "fgb_metrics_add_records", "fgb_metrics_finish", "fgb_metrics_table",
     "fgb_metrics_stats", "fgb_metrics_last_timing",
+    "fgb_zipper_records", "fgb_host_zipper_records", "fgb_host_free_buffer", "fgb_zipper_last_timing",
 )
 
 _lib = None
@@ -592,6 +604,16 @@ def load() -> C.CDLL:
     lib.fgb_metrics_stats.restype = C.c_int32
     lib.fgb_metrics_last_timing.argtypes = [vp, vp]
     lib.fgb_metrics_last_timing.restype = C.c_int32
+    lib.fgb_zipper_records.argtypes = [vp, C.POINTER(FgbZipperOptions), vp, vp, u64, vp, vp, u64, C.c_int,
+                                       C.POINTER(vp), C.POINTER(u64), C.POINTER(u64), vp, C.POINTER(u64)]
+    lib.fgb_zipper_records.restype = C.c_int32
+    lib.fgb_host_zipper_records.argtypes = [C.POINTER(FgbZipperOptions), vp, vp, u64, vp, vp, u64, C.c_int,
+                                            C.POINTER(vp), C.POINTER(u64), C.POINTER(u64), vp, C.POINTER(u64)]
+    lib.fgb_host_zipper_records.restype = C.c_int32
+    lib.fgb_host_free_buffer.argtypes = [vp]
+    lib.fgb_host_free_buffer.restype = None
+    lib.fgb_zipper_last_timing.argtypes = [vp, vp]
+    lib.fgb_zipper_last_timing.restype = C.c_int32
     lib.fgb_struct_size.argtypes = [C.c_uint32]
     lib.fgb_struct_size.restype = C.c_uint32
     _lib = lib

@@ -1277,11 +1277,61 @@ fgb_status fgb_metrics_stats(const fgb_metrics* m, uint64_t stats[FGB_METRICS_NS
  * The staging buffers are at most 64 MiB; FGB_METRICS_STAGE_BYTES (at least 4096) lowers that, read on each call. */
 fgb_status fgb_metrics_last_timing(const fgb_metrics* m, double ms[4]);
 
+/* ---- `fgumi zipper` on raw records (src/lib/commands/zipper.rs process_raw :826-941, merge_raw :373-521,
+ * Template::fix_mate_info in template.rs:411-710): the mapped records of each template get their mate fields, TLEN,
+ * MQ / MC / ms, the unmapped read's tags (reversed or reverse-complemented on the reverse strand), its QC flag, AS / XS
+ * in the smallest signed type and, on secondary and supplementary records, the tc tag.  BAM records only; SAM text,
+ * --restore-unconverted-bases and stdin are not offered. */
+typedef struct fgb_zipper_options {
+  uint8_t exclude_missing_reads;     /* drop (and count) unmapped templates with no mapped template               */
+  uint8_t skip_pa_tags;              /* no tc tag on secondary / supplementary records (--skip-pa-tags)           */
+  uint8_t restore_unconverted_bases; /* not offered: non-zero gives FGB_ERR_INVALID_ARG                           */
+  uint8_t reserved[1];
+  uint32_t n_threads;                /* host threads (staging copies); 0 or 1 = the calling thread                 */
+  uint64_t device_bytes;             /* device-memory budget of one run of templates; 0 = from cudaMemGetInfo     */
+  uint64_t n_remove, n_reverse, n_revcomp;        /* the expanded tag lists (a named set like Consensus expanded   */
+  const char (*tags_to_remove)[2];                /* by the caller): two bytes per name, no NUL                     */
+  const char (*tags_to_reverse)[2];
+  const char (*tags_to_revcomp)[2];
+} fgb_zipper_options;
+enum { FGB_ZSTAT_MERGED = 0, FGB_ZSTAT_UNMAPPED_ONLY = 1, FGB_ZSTAT_EXCLUDED = 2, FGB_ZSTAT_RECORDS_OUT = 3,
+       FGB_ZIPPER_NSTATS = 4 };
+/* Zips n_unmapped unmapped records (whole QNAME runs) with the mapped records not yet consumed (whole QNAME runs, in
+ * the same name order; record i of a stream = records[off[i] .. off[i+1]), no block_size prefix).  Stateless.  Each
+ * unmapped template (Template::from_records order) is merged with the next mapped template when their names are
+ * equal as bytes -- the mapped records come out in template order -- else emitted unchanged (or, with
+ * exclude_missing_reads, dropped).  *mapped_consumed = the mapped records the join used; without last_call the
+ * rest are the caller's to pass again, with last_call a mapped template left over fails the call.  Output: *out, a
+ * library-owned [u32 block_size][record] stream valid until the next call on `h`, and stats[FGB_ZSTAT_*].
+ * Synchronous.  Errors fail the call and emit nothing; *bad_record names the first bad record met in join order,
+ * counting the unmapped records as 0 .. n_unmapped - 1 and mapped record j as n_unmapped + j: a record shorter than
+ * 32 bytes, with truncated fields or an aux area that does not parse to its end (FGB_ERR_LAYOUT), a record carrying
+ * one tag twice, a mapped record with a CIGAR op code past 8, a template with two primary R1s or R2s, a mapped template
+ * left over with last_call (FGB_ERR_INVALID_ARG).  A tag list entry with a NUL byte or restore_unconverted_bases
+ * give FGB_ERR_INVALID_ARG.  One call runs on the handle's one GPU. */
+fgb_status fgb_zipper_records(fgb_handle* h, const fgb_zipper_options* opt, const uint8_t* unmapped,
+                              const uint64_t* u_off, uint64_t n_unmapped, const uint8_t* mapped, const uint64_t* m_off,
+                              uint64_t n_mapped, int last_call, const uint8_t** out, uint64_t* out_len,
+                              uint64_t* mapped_consumed, uint64_t stats[FGB_ZIPPER_NSTATS], uint64_t* bad_record);
+/* The same on host threads, with the same per-record rules (no device; for tests, there is no CPU zipper): *out is a
+ * malloc'ed stream the caller frees with fgb_host_free_buffer. */
+fgb_status fgb_host_zipper_records(const fgb_zipper_options* opt, const uint8_t* unmapped, const uint64_t* u_off,
+                                   uint64_t n_unmapped, const uint8_t* mapped, const uint64_t* m_off, uint64_t n_mapped,
+                                   int last_call, uint8_t** out, uint64_t* out_len, uint64_t* mapped_consumed,
+                                   uint64_t stats[FGB_ZIPPER_NSTATS], uint64_t* bad_record);
+void fgb_host_free_buffer(void* p);
+/* Where the last fgb_zipper_records on `h` spent its time, in ms, summed over its runs: [0] upload, [1] size pass,
+ * [2] offset scan, [3] write pass, [4] download (with the output's growth), [5] host work (checks, join, template
+ * table, allocations).  [1]-[3] are CUDA events.  The staging buffers are at most 64 MiB; FGB_ZIPPER_STAGE_BYTES (at
+ * least 4096) lowers that, read on every call. */
+fgb_status fgb_zipper_last_timing(const fgb_handle* h, double ms[6]);
+
 /* sizeof() of the ABI structs as this library was compiled, so a binding can check its own layout:
  * 0 fgb_caller_options, 1 fgb_filter_params, 2 fgb_submit_options, 3 fgb_raw_columns,
  * 4 fgb_raw_read, 5 fgb_batch, 6 fgb_codec_params, 7 fgb_params, 8 fgb_duplex_filter_params,
  * 9 fgb_record_columns, 10 fgb_umi_options, 11 fgb_group_options, 12 fgb_sort_options, 13 fgb_dedup_options,
- * 14 fgb_record_filter_options, 15 fgb_metrics_options, 16 fgb_metrics_template; 0 for an unknown id. */
+ * 14 fgb_record_filter_options, 15 fgb_metrics_options, 16 fgb_metrics_template, 17 fgb_zipper_options; 0 for an
+ * unknown id. */
 uint32_t fgb_struct_size(uint32_t id);
 
 #ifdef __cplusplus
