@@ -1655,20 +1655,6 @@ fgb_status umi_assign_impl(fgb_handle* h, const fgb_umi_options& o, const uint8_
   return FGB_OK;
 }
 
-// No exception crosses the ABI: host allocations (and thread creation) that fail become status codes.
-template <class F>
-fgb_status umi_guard(fgb_handle* h, F&& f) {
-  try {
-    return f();
-  } catch (const std::bad_alloc&) {
-    h->last_error = "fgb_umi_assign: out of host memory";
-    return FGB_ERR_NOMEM;
-  } catch (const std::exception& e) {
-    h->last_error = std::string("fgb_umi_assign: ") + e.what();
-    return FGB_ERR_NOMEM;
-  }
-}
-
 }  // namespace
 
 extern "C" {
@@ -1682,7 +1668,7 @@ fgb_status fgb_umi_assign(fgb_handle* h, const fgb_umi_options* opt, const uint8
   const std::string bad = fgb_umi::check_options(*opt);
   if (!bad.empty()) { h->last_error = "fgb_umi_assign: " + bad; return FGB_ERR_INVALID_ARG; }
   if (h->submit_pending) { h->last_error = "fgb_umi_assign: a submit has not been waited on"; return FGB_ERR_BUSY; }
-  return umi_guard(h, [&] {
+  return fgb::link::guarded(&h->last_error, "fgb_umi_assign", [&] {
     return umi_assign_impl(h, *opt, umis, umi_off, n_umis, call_off, n_calls, group_off, n_groups, ids, kinds,
                            group_mi_count);
   });
@@ -1701,7 +1687,8 @@ fgb_status fgb_umi_edges(fgb_handle* h, const fgb_umi_options* opt, const uint8_
   const std::string bad = fgb_umi::check_options(*opt);
   if (!bad.empty()) { h->last_error = "fgb_umi_edges: " + bad; return FGB_ERR_INVALID_ARG; }
   if (h->submit_pending) { h->last_error = "fgb_umi_edges: a submit has not been waited on"; return FGB_ERR_BUSY; }
-  return umi_guard(h, [&]() -> fgb_status {
+  // reports as "fgb_umi_assign: ..." like the assignment whose edge phase this is
+  return fgb::link::guarded(&h->last_error, "fgb_umi_assign", [&]() -> fgb_status {
     const uint64_t call_off[2] = {0, n_umis}, group_off[2] = {0, 1};
     FGB_TRY(umi_check_layout(h, umi_off, n_umis, call_off, 1, group_off, 1));
     std::vector<fgb_umi::Call> calls;
@@ -1992,7 +1979,7 @@ fgb_status fgb_record_quality_scores(fgb_handle* h, const uint8_t* records, cons
       h->last_error = "fgb_record_quality_scores: record " + std::to_string(i) + " is shorter than 32 bytes";
       return FGB_ERR_LAYOUT;
     }
-  try {
+  return fgb::link::guarded(&h->last_error, "fgb_record_quality_scores", [&] {
     std::vector<const uint8_t*> rp(n_records);
     std::vector<uint64_t> rl(n_records);
     for (uint64_t i = 0; i < n_records; ++i) { rp[i] = records + rec_off[i]; rl[i] = rec_off[i + 1] - rec_off[i]; }
@@ -2001,10 +1988,7 @@ fgb_status fgb_record_quality_scores(fgb_handle* h, const uint8_t* records, cons
     const fgb_status st = fgb::dedupdev::quality_scores(h, n_records, rp.data(), rl.data(), 1, scores, &kernel_ms, &err);
     if (st != FGB_OK) h->last_error = "fgb_record_quality_scores: " + err;
     return st;
-  } catch (const std::bad_alloc&) {
-    h->last_error = "fgb_record_quality_scores: out of host memory";
-    return FGB_ERR_NOMEM;
-  }
+  });
 }
 
 }  // extern "C"

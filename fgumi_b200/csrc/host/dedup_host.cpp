@@ -27,6 +27,7 @@ namespace {
 using fgb::bam::View;
 namespace bam = fgb::bam;
 using namespace fgb::grp;
+using fgb::link::guarded;
 using fgb::link::ms_since;
 
 constexpr uint16_t kDuplicate = 0x400;
@@ -59,9 +60,7 @@ struct fgb_deduper {
   uint64_t stats[FGB_DEDUP_NSTATS] = {};
   std::map<uint64_t, uint64_t> family_sizes;
   std::string last_error;
-  bool batch_ready = false;           // the UMI batch of the queue (fgb_deduper_pending), built on demand
-  std::vector<uint8_t> b_umis;
-  std::vector<uint64_t> b_umi_off, b_call_off, b_group_off;
+  UmiBatch batch;                     // the queue's UMI batch (fgb_deduper_pending)
   std::vector<uint8_t> out;
   double timing[7] = {0, 0, 0, 0, 0, 0, 0};   // fgb_deduper_last_timing
 };
@@ -149,20 +148,6 @@ std::string prepare_group(const fgb_deduper& d, const uint8_t* records, const ui
   return split_and_umis(d.umi, d.opt.no_umi, d.opt.umi_tag, gp->tpls.size(),
                         [&](size_t t) { return gp->tpls[t].r1 >= 0 ? &pv[gp->tpls[t].r1] : nullptr; },
                         [&](size_t t) { return gp->tpls[t].r2 >= 0 ? &pv[gp->tpls[t].r2] : nullptr; }, &gp->c);
-}
-
-void build_batch(fgb_deduper* d) {
-  if (d->batch_ready) return;
-  d->b_umis.clear(); d->b_umi_off.assign(1, 0); d->b_call_off.assign(1, 0); d->b_group_off.assign(1, 0);
-  for (const DGroup& gp : d->queue) {
-    const uint64_t base = d->b_umis.size();
-    d->b_umis.insert(d->b_umis.end(), gp.c.umis.begin(), gp.c.umis.end());
-    for (uint64_t e : gp.c.umi_end) d->b_umi_off.push_back(base + e);
-    const uint64_t ub = d->b_call_off.back();
-    for (uint32_t e : gp.c.call_end) d->b_call_off.push_back(ub + e);
-    d->b_group_off.push_back(d->b_call_off.size() - 1);
-  }
-  d->batch_ready = true;
 }
 
 // find_tag_type (fgumi-raw-bam): whether the record has an aux entry `tag` of any type
@@ -257,25 +242,18 @@ void emit_group(const fgb_deduper& d, const DGroup& gp, const uint64_t* ids, con
 fgb_status finish_flush(fgb_deduper* d, const uint64_t* ids, const uint8_t* kinds, const uint64_t* mi_count,
                         const uint32_t* scores, const uint8_t** out, uint64_t* out_len, uint64_t* n_records) {
   const uint64_t ng = d->queue.size();
-  std::vector<uint64_t> base(ng);
+  std::vector<uint64_t> base;
   uint64_t next = d->stats[FGB_DSTAT_NEXT_MI];
-  for (uint64_t b = 0; b < ng; ++b) {   // the MI counter advances by max(id) + 1 per group (:791-797, 1123-1133)
-    base[b] = next;
-    if (next + mi_count[b] < next) { d->last_error = "fgb_deduper_flush: MI counter overflow"; return FGB_ERR_INVALID_ARG; }
-    next += mi_count[b];
+  if (!mi_bases(mi_count, ng, &next, &base)) {
+    d->last_error = "fgb_deduper_flush: MI counter overflow";
+    return FGB_ERR_INVALID_ARG;
   }
   std::vector<DedupOut> outs(ng);
   fgb_umi::parallel_for(ng, d->opt.umi.n_threads, [&](uint64_t b) {
-    const uint64_t u0 = d->b_call_off[d->b_group_off[b]];
+    const uint64_t u0 = d->batch.call_off[d->batch.group_off[b]];
     emit_group(*d, d->queue[b], ids + u0, kinds + u0, scores + u0, base[b], &outs[b]);
   });
-  std::vector<uint64_t> at(ng + 1, 0);
-  uint64_t recs = 0;
-  for (uint64_t b = 0; b < ng; ++b) { at[b + 1] = at[b] + outs[b].bytes.size(); recs += outs[b].n_records; }
-  d->out.resize(at[ng]);
-  fgb_umi::parallel_for(ng, d->opt.umi.n_threads, [&](uint64_t b) {
-    if (!outs[b].bytes.empty()) std::memcpy(d->out.data() + at[b], outs[b].bytes.data(), outs[b].bytes.size());
-  });
+  const uint64_t recs = concat_outputs(outs, d->opt.umi.n_threads, &d->out);
   for (uint64_t b = 0; b < ng; ++b) {
     for (uint64_t f : outs[b].families) d->family_sizes[f]++;
     for (int k = 0; k <= FGB_DSTAT_MISSING_TC_TAG; ++k) d->stats[k] += outs[b].m[k];
@@ -284,23 +262,11 @@ fgb_status finish_flush(fgb_deduper* d, const uint64_t* ids, const uint8_t* kind
   d->stats[FGB_DSTAT_NEXT_MI] = next;
   d->stats[FGB_DSTAT_RECORDS_OUT] += recs;
   d->queue.clear();
-  d->batch_ready = false;
+  d->batch.ready = false;
   *out = d->out.data();
   *out_len = d->out.size();
   *n_records = recs;
   return FGB_OK;
-}
-
-template <class F>
-fgb_status guard(fgb_deduper* d, const char* where, F&& f) {
-  try {
-    return f();
-  } catch (const std::bad_alloc&) {
-    d->last_error = std::string(where) + ": out of host memory";
-  } catch (const std::exception& e) {
-    d->last_error = std::string(where) + ": " + e.what();
-  }
-  return FGB_ERR_NOMEM;
 }
 
 }  // namespace
@@ -321,15 +287,8 @@ fgb_status fgb_deduper_create(int device, const fgb_dedup_options* opt, fgb_dedu
   d->opt = *opt;
   d->umi = u;
   d->stats[FGB_DSTAT_NEXT_MI] = opt->first_mi;
-  if (device != FGB_DEVICE_NONE) {
-    fgb_params p{};
-    p.error_rate_pre_umi = 45;
-    p.error_rate_post_umi = 40;
-    p.min_consensus_base_quality = 40;
-    p.min_reads = 1;
-    const fgb_status st = fgb_create(device, &p, &d->h);
-    if (st != FGB_OK) return st;
-  }
+  const fgb_status st = open_handle(device, &d->h);
+  if (st != FGB_OK) return st;
   *out = d.release();
   return FGB_OK;
 }
@@ -341,37 +300,20 @@ void fgb_deduper_destroy(fgb_deduper* d) {
 }
 
 size_t fgb_deduper_last_error(const fgb_deduper* d, char* buf, size_t buf_len) {
-  if (!d) return 0;
-  if (buf && buf_len) {
-    const size_t n = std::min(buf_len - 1, d->last_error.size());
-    std::memcpy(buf, d->last_error.data(), n);
-    buf[n] = 0;
-  }
-  return d->last_error.size();
+  return d ? copy_error(d->last_error, buf, buf_len) : 0;
 }
 
 fgb_status fgb_deduper_add_groups(fgb_deduper* d, const uint8_t* records, const uint64_t* rec_off,
                                   const uint64_t* group_rec, uint64_t n_groups) {
   if (!d || !group_rec || (n_groups && (!records || !rec_off))) return FGB_ERR_INVALID_ARG;
-  return guard(d, "fgb_deduper_add_groups", [&]() -> fgb_status {
-    for (uint64_t x = 0; x < n_groups; ++x)
-      if (group_rec[x + 1] < group_rec[x]) { d->last_error = "fgb_deduper_add_groups: group_rec descends"; return FGB_ERR_LAYOUT; }
-    const uint64_t r0 = n_groups ? group_rec[0] : 0, r1 = n_groups ? group_rec[n_groups] : 0;
-    for (uint64_t i = r0; i < r1; ++i)
-      if (!record_ok(records, rec_off, i)) {
-        d->last_error = "fgb_deduper_add_groups: record " + std::to_string(i) + " is malformed";
-        return FGB_ERR_LAYOUT;
-      }
-    std::vector<DGroup> prep(n_groups);
-    std::vector<std::string> err(n_groups);
-    fgb_umi::parallel_for(n_groups, d->opt.umi.n_threads, [&](uint64_t x) {
-      err[x] = prepare_group(*d, records, rec_off, group_rec[x], group_rec[x + 1], &prep[x]);
-    });
-    for (uint64_t x = 0; x < n_groups; ++x)   // an assignment error fails the command (dedup.rs:717-719)
-      if (!err[x].empty()) {
-        d->last_error = "fgb_deduper_add_groups: position group " + std::to_string(x) + ": " + err[x];
-        return FGB_ERR_INVALID_ARG;
-      }
+  static const char kWho[] = "fgb_deduper_add_groups";
+  return guarded(&d->last_error, kWho, [&]() -> fgb_status {
+    std::vector<DGroup> prep;   // an assignment error fails the command (dedup.rs:717-719)
+    const fgb_status st = prepare_groups(
+        kWho, records, rec_off, group_rec, n_groups, d->opt.umi.n_threads,
+        [&](uint64_t b, uint64_t e, DGroup* gp) { return prepare_group(*d, records, rec_off, b, e, gp); }, &prep,
+        &d->last_error);
+    if (st != FGB_OK) return st;
     d->queue.reserve(d->queue.size() + n_groups);
     for (auto& gp : prep) {
       for (int k = 0; k < 6; ++k) d->stats[FGB_DSTAT_FILTER_TOTAL + k] += gp.filter[k];
@@ -379,7 +321,7 @@ fgb_status fgb_deduper_add_groups(fgb_deduper* d, const uint8_t* records, const 
       if (gp.tpls.empty()) continue;   // nothing of it reaches the output (:696-704)
       d->queue.push_back(std::move(gp));
     }
-    d->batch_ready = false;
+    d->batch.ready = false;
     return FGB_OK;
   });
 }
@@ -388,15 +330,9 @@ fgb_status fgb_deduper_pending(fgb_deduper* d, const uint8_t** umis, const uint6
                                const uint64_t** call_off, uint64_t* n_calls, const uint64_t** group_off,
                                uint64_t* n_groups) {
   if (!d || !umis || !umi_off || !n_umis || !call_off || !n_calls || !group_off || !n_groups) return FGB_ERR_INVALID_ARG;
-  return guard(d, "fgb_deduper_pending", [&]() -> fgb_status {
-    build_batch(d);
-    *umis = d->b_umis.data();
-    *umi_off = d->b_umi_off.data();
-    *n_umis = d->b_umi_off.size() - 1;
-    *call_off = d->b_call_off.data();
-    *n_calls = d->b_call_off.size() - 1;
-    *group_off = d->b_group_off.data();
-    *n_groups = d->b_group_off.size() - 1;
+  return guarded(&d->last_error, "fgb_deduper_pending", [&]() -> fgb_status {
+    d->batch.build(d->queue);
+    d->batch.pending(umis, umi_off, n_umis, call_off, n_calls, group_off, n_groups);
     return FGB_OK;
   });
 }
@@ -404,9 +340,9 @@ fgb_status fgb_deduper_pending(fgb_deduper* d, const uint8_t** umis, const uint6
 fgb_status fgb_deduper_flush(fgb_deduper* d, const uint8_t** out, uint64_t* out_len, uint64_t* n_records) {
   if (!d || !out || !out_len || !n_records) return FGB_ERR_INVALID_ARG;
   if (!d->h) { d->last_error = "fgb_deduper_flush: a planning-only deduper has no device"; return FGB_ERR_NO_DEVICE; }
-  return guard(d, "fgb_deduper_flush", [&]() -> fgb_status {
-    build_batch(d);
-    const uint64_t n = d->b_umi_off.size() - 1, nc = d->b_call_off.size() - 1, ng = d->b_group_off.size() - 1;
+  return guarded(&d->last_error, "fgb_deduper_flush", [&]() -> fgb_status {
+    d->batch.build(d->queue);
+    const uint64_t n = d->batch.n_umis(), ng = d->batch.n_groups();
     // the primary records of every batch entry, R1 then R2 (score_template, dedup.rs:230-249)
     std::vector<const uint8_t*> rp;
     std::vector<uint64_t> rl, first(n + 1);
@@ -426,36 +362,23 @@ fgb_status fgb_deduper_flush(fgb_deduper* d, const uint8_t** out, uint64_t* out_
     std::vector<uint32_t> rscore(rp.size() + 1);
     std::vector<uint64_t> ids(n + 1), counts(ng + 1);
     std::vector<uint8_t> kinds(n + 1);
-    static const uint8_t kNoBytes = 0;   // every UMI empty (no_umi): the ABI still wants a pointer
-    const uint8_t* umis = d->b_umis.empty() ? &kNoBytes : d->b_umis.data();
     // the score phase runs on its own thread and stream while the assignment runs here
     fgb_status score_st = FGB_OK;
     float kernel_ms = 0.f;
     double score_ms = 0.0;
     std::string score_err;
-    std::thread scorer([&] {   // nothing may escape a std::thread: failures become a status, as in guard()
+    std::thread scorer([&] {
       const auto t0 = std::chrono::steady_clock::now();
-      try {
-        score_st = fgb::dedupdev::quality_scores(d->h, rp.size(), rp.data(), rl.data(), d->opt.umi.n_threads,
-                                                 rscore.data(), &kernel_ms, &score_err);
-      } catch (const std::bad_alloc&) {
-        score_st = FGB_ERR_NOMEM;
-        score_err = "template scores: out of host memory";
-      } catch (const std::exception& e) {
-        score_st = FGB_ERR_NOMEM;
-        score_err = std::string("template scores: ") + e.what();
-      }
+      score_st = guarded(&score_err, "template scores", [&] {
+        return fgb::dedupdev::quality_scores(d->h, rp.size(), rp.data(), rl.data(), d->opt.umi.n_threads,
+                                             rscore.data(), &kernel_ms, &score_err);
+      });
       score_ms = ms_since(t0);
     });
-    const fgb_status st = fgb_umi_assign(d->h, &d->umi, umis, d->b_umi_off.data(), n, d->b_call_off.data(), nc,
-                                         d->b_group_off.data(), ng, ids.data(), kinds.data(), counts.data());
+    const fgb_status st = d->batch.assign(d->h, d->umi, "fgb_deduper_flush", ids.data(), kinds.data(), counts.data(),
+                                          &d->last_error);
     scorer.join();
-    if (st != FGB_OK) {
-      std::string e(fgb_last_error(d->h, nullptr, 0), '\0');
-      fgb_last_error(d->h, &e[0], e.size() + 1);
-      d->last_error = "fgb_deduper_flush: " + e;
-      return st;
-    }
+    if (st != FGB_OK) return st;
     if (score_st != FGB_OK) { d->last_error = "fgb_deduper_flush: " + score_err; return score_st; }
     fgb_umi_last_timing(d->h, d->timing);
     d->timing[4] = score_ms;
@@ -474,9 +397,9 @@ fgb_status fgb_deduper_flush_with_ids(fgb_deduper* d, const uint64_t* ids, const
                                       const uint64_t* group_mi_count, const uint32_t* scores, const uint8_t** out,
                                       uint64_t* out_len, uint64_t* n_records) {
   if (!d || !out || !out_len || !n_records) return FGB_ERR_INVALID_ARG;
-  return guard(d, "fgb_deduper_flush_with_ids", [&]() -> fgb_status {
-    build_batch(d);
-    const uint64_t n = d->b_umi_off.size() - 1, ng = d->b_group_off.size() - 1;
+  return guarded(&d->last_error, "fgb_deduper_flush_with_ids", [&]() -> fgb_status {
+    d->batch.build(d->queue);
+    const uint64_t n = d->batch.n_umis(), ng = d->batch.n_groups();
     if ((n && (!ids || !kinds || !scores)) || (ng && !group_mi_count)) return FGB_ERR_INVALID_ARG;
     for (uint64_t u = 0; u < n; ++u)
       if (kinds[u] > FGB_MOL_B) { d->last_error = "fgb_deduper_flush_with_ids: unknown kind"; return FGB_ERR_INVALID_ARG; }
@@ -492,12 +415,7 @@ fgb_status fgb_deduper_stats(const fgb_deduper* d, uint64_t stats[FGB_DEDUP_NSTA
 
 fgb_status fgb_deduper_histogram(const fgb_deduper* d, uint64_t* sizes, uint64_t* counts, uint64_t cap, uint64_t* n) {
   if (!d || !n) return FGB_ERR_INVALID_ARG;
-  *n = d->family_sizes.size();
-  if (cap < d->family_sizes.size()) return FGB_OK;
-  if (d->family_sizes.size() && (!sizes || !counts)) return FGB_ERR_INVALID_ARG;
-  uint64_t i = 0;
-  for (const auto& [s, c] : d->family_sizes) { sizes[i] = s; counts[i] = c; ++i; }
-  return FGB_OK;
+  return copy_histogram(d->family_sizes, sizes, counts, cap, n);
 }
 
 fgb_status fgb_deduper_last_timing(const fgb_deduper* d, double ms[7]) {

@@ -391,7 +391,7 @@ fgb_status fgb_filter_records(fgb_handle* h, const fgb_record_filter_options* op
     return FGB_ERR_INVALID_ARG;
   }
   if (hi.busy) { *hi.last_error = "fgb_filter_records: a submit has not been waited on"; return FGB_ERR_BUSY; }
-  const fgb_status st = link::guarded(hi, "fgb_filter_records", [&]() -> fgb_status {
+  const fgb_status st = link::guarded(hi.last_error, "fgb_filter_records", [&]() -> fgb_status {
     hi.kept->clear();
     hi.rejects->clear();
     return n_records ? filter_impl(hi, *opt, ref, std::string_view(header_text ? header_text : "", header_len), records,

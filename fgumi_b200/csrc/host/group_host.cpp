@@ -17,6 +17,7 @@
 #include "../../../include/fgumi_b200.h"
 #include "bam.h"
 #include "group_rules.h"
+#include "record_link.h"
 #include "umi_host.h"
 
 namespace {
@@ -24,6 +25,7 @@ namespace {
 using fgb::bam::View;
 namespace bam = fgb::bam;
 using namespace fgb::grp;
+using fgb::link::guarded;
 
 // ---- position grouping (unified_pipeline/bam.rs:415-499, base.rs:1375-1436, grouper.rs:406-588) ----------------
 struct PosKey {
@@ -81,10 +83,7 @@ struct fgb_grouper {
   uint64_t stats[FGB_GROUP_NSTATS] = {};
   std::map<uint64_t, uint64_t> family_sizes, group_sizes;
   std::string last_error;
-  // the UMI batch of the queue (fgb_grouper_pending), built on demand
-  bool batch_ready = false;
-  std::vector<uint8_t> b_umis;
-  std::vector<uint64_t> b_umi_off, b_call_off, b_group_off, b_group_of;   // b_group_of: queue index per batch group
+  UmiBatch batch;               // the queue's UMI batch (fgb_grouper_pending)
   std::vector<uint8_t> out;
   double timing[5] = {0, 0, 0, 0, 0};   // fgb_grouper_last_timing
 };
@@ -127,23 +126,18 @@ std::string prepare_group(const fgb_grouper& g, const uint8_t* records, const ui
   std::vector<View> views;
   views.reserve(e - b);
   for (uint64_t i = b; i < e; ++i) views.emplace_back(records + rec_off[i], rec_off[i + 1] - rec_off[i]);
-  uint64_t i = 0;
   const uint64_t n = e - b;
-  while (i < n) {
+  std::vector<uint64_t> lists[4], order;
+  for (uint64_t i = 0; i < n;) {
     uint64_t j = i + 1;
     const std::string_view name = read_name(views[i]);
     while (j < n && read_name(views[j]) == name) ++j;
-    int64_t r1 = -1, r2 = -1;
-    for (uint64_t k = i; k < j; ++k) {
-      const uint16_t f = views[k].flags();
-      const bool is_r1 = !(f & bam::kPaired) || (f & bam::kFirst);
-      if (f & (bam::kSecondary | bam::kSupplementary)) continue;
-      int64_t& slot = is_r1 ? r1 : r2;
-      if (slot >= 0)
-        return std::string("Multiple non-secondary, non-supplemental ") + (is_r1 ? "R1" : "R2") + " records for read '" +
-               std::string(name) + "'";
-      slot = static_cast<int64_t>(k);
-    }
+    int64_t r1, r2;
+    uint64_t dup;
+    order.clear();
+    const std::string err = template_order(i, j, [&](uint64_t k) { return views[k].flags(); }, name, lists, &order,
+                                           &r1, &r2, &dup);
+    if (!err.empty()) return err;
     const View* v1 = r1 >= 0 ? &views[r1] : nullptr;
     const View* v2 = r2 >= 0 ? &views[r2] : nullptr;
     if (filter_template(g, v1, v2, gp->filter)) {
@@ -178,31 +172,14 @@ std::string prepare_group(const fgb_grouper& g, const uint8_t* records, const ui
   return "";
 }
 
-void build_batch(fgb_grouper* g) {
-  if (g->batch_ready) return;
-  g->b_umis.clear(); g->b_umi_off.assign(1, 0); g->b_call_off.assign(1, 0); g->b_group_off.assign(1, 0);
-  g->b_group_of.clear();
-  for (uint64_t q = 0; q < g->queue.size(); ++q) {
-    const GroupPrep& gp = g->queue[q];
-    if (gp.dropped || gp.tpls.empty()) continue;
-    const uint64_t base = g->b_umis.size();
-    g->b_umis.insert(g->b_umis.end(), gp.c.umis.begin(), gp.c.umis.end());
-    for (uint64_t e : gp.c.umi_end) g->b_umi_off.push_back(base + e);
-    const uint64_t ub = g->b_call_off.back();
-    for (uint32_t e : gp.c.call_end) g->b_call_off.push_back(ub + e);
-    g->b_group_off.push_back(g->b_call_off.size() - 1);
-    g->b_group_of.push_back(q);
-  }
-  g->batch_ready = true;
-}
-
 struct GroupOut {
   std::vector<uint8_t> bytes;
   std::vector<uint64_t> families;   // template count of each molecule, in output order
   uint64_t n_records = 0;
 };
 
-// process_and_write_position_group after the assignment (group.rs:1524-1592, 1650-1682) for batch group `bg`.
+// process_and_write_position_group after the assignment (group.rs:1524-1592, 1650-1682) for queued group `gp`;
+// ids / kinds indexed like its batch entries (gp.c.order).
 void emit_group(const fgb_grouper& g, const GroupPrep& gp, const uint64_t* ids, const uint8_t* kinds, uint64_t base_mi,
                 GroupOut* go) {
   const size_t nt = gp.tpls.size();
@@ -244,26 +221,19 @@ void emit_group(const fgb_grouper& g, const GroupPrep& gp, const uint64_t* ids, 
 
 fgb_status finish_flush(fgb_grouper* g, const uint64_t* ids, const uint8_t* kinds, const uint64_t* mi_count,
                         const uint8_t** out, uint64_t* out_len, uint64_t* n_records) {
-  const uint64_t ng = g->b_group_of.size();
-  std::vector<uint64_t> base(ng);
+  const uint64_t ng = g->queue.size();
+  std::vector<uint64_t> base;
   uint64_t next = g->stats[FGB_GSTAT_NEXT_MI];
-  for (uint64_t b = 0; b < ng; ++b) {   // the MI counter advances by max(id) + 1 per group (:1569-1575)
-    base[b] = next;
-    if (next + mi_count[b] < next) { g->last_error = "fgb_grouper_flush: MI counter overflow"; return FGB_ERR_INVALID_ARG; }
-    next += mi_count[b];
+  if (!mi_bases(mi_count, ng, &next, &base)) {
+    g->last_error = "fgb_grouper_flush: MI counter overflow";
+    return FGB_ERR_INVALID_ARG;
   }
   std::vector<GroupOut> outs(ng);
   fgb_umi::parallel_for(ng, g->opt.umi.n_threads, [&](uint64_t b) {
-    const uint64_t u0 = g->b_call_off[g->b_group_off[b]];
-    emit_group(*g, g->queue[g->b_group_of[b]], ids + u0, kinds + u0, base[b], &outs[b]);
+    const uint64_t u0 = g->batch.call_off[g->batch.group_off[b]];
+    emit_group(*g, g->queue[b], ids + u0, kinds + u0, base[b], &outs[b]);
   });
-  std::vector<uint64_t> at(ng + 1, 0);
-  uint64_t recs = 0;
-  for (uint64_t b = 0; b < ng; ++b) { at[b + 1] = at[b] + outs[b].bytes.size(); recs += outs[b].n_records; }
-  g->out.resize(at[ng]);
-  fgb_umi::parallel_for(ng, g->opt.umi.n_threads, [&](uint64_t b) {
-    if (!outs[b].bytes.empty()) std::memcpy(g->out.data() + at[b], outs[b].bytes.data(), outs[b].bytes.size());
-  });
+  const uint64_t recs = concat_outputs(outs, g->opt.umi.n_threads, &g->out);
   for (uint64_t b = 0; b < ng; ++b) {
     for (uint64_t f : outs[b].families) g->family_sizes[f]++;
     if (!outs[b].families.empty()) g->group_sizes[outs[b].families.size()]++;
@@ -271,23 +241,11 @@ fgb_status finish_flush(fgb_grouper* g, const uint64_t* ids, const uint8_t* kind
   g->stats[FGB_GSTAT_NEXT_MI] = next;
   g->stats[FGB_GSTAT_RECORDS_OUT] += recs;
   g->queue.clear();
-  g->batch_ready = false;
+  g->batch.ready = false;
   *out = g->out.data();
   *out_len = g->out.size();
   *n_records = recs;
   return FGB_OK;
-}
-
-template <class F>
-fgb_status guard(fgb_grouper* g, const char* where, F&& f) {
-  try {
-    return f();
-  } catch (const std::bad_alloc&) {
-    g->last_error = std::string(where) + ": out of host memory";
-  } catch (const std::exception& e) {
-    g->last_error = std::string(where) + ": " + e.what();
-  }
-  return FGB_ERR_NOMEM;
 }
 
 }  // namespace
@@ -413,15 +371,8 @@ fgb_status fgb_grouper_create(int device, const fgb_group_options* opt, fgb_grou
   g->opt = *opt;
   g->umi = u;
   g->stats[FGB_GSTAT_NEXT_MI] = opt->first_mi;
-  if (device != FGB_DEVICE_NONE) {
-    fgb_params p{};
-    p.error_rate_pre_umi = 45;
-    p.error_rate_post_umi = 40;
-    p.min_consensus_base_quality = 40;
-    p.min_reads = 1;
-    const fgb_status st = fgb_create(device, &p, &g->h);
-    if (st != FGB_OK) return st;
-  }
+  const fgb_status st = open_handle(device, &g->h);
+  if (st != FGB_OK) return st;
   *out = g.release();
   return FGB_OK;
 }
@@ -433,37 +384,20 @@ void fgb_grouper_destroy(fgb_grouper* g) {
 }
 
 size_t fgb_grouper_last_error(const fgb_grouper* g, char* buf, size_t buf_len) {
-  if (!g) return 0;
-  if (buf && buf_len) {
-    const size_t n = std::min(buf_len - 1, g->last_error.size());
-    std::memcpy(buf, g->last_error.data(), n);
-    buf[n] = 0;
-  }
-  return g->last_error.size();
+  return g ? copy_error(g->last_error, buf, buf_len) : 0;
 }
 
 fgb_status fgb_grouper_add_groups(fgb_grouper* g, const uint8_t* records, const uint64_t* rec_off,
                                   const uint64_t* group_rec, uint64_t n_groups) {
   if (!g || !group_rec || (n_groups && (!records || !rec_off))) return FGB_ERR_INVALID_ARG;
-  return guard(g, "fgb_grouper_add_groups", [&]() -> fgb_status {
-    for (uint64_t x = 0; x < n_groups; ++x)
-      if (group_rec[x + 1] < group_rec[x]) { g->last_error = "fgb_grouper_add_groups: group_rec descends"; return FGB_ERR_LAYOUT; }
-    const uint64_t r0 = n_groups ? group_rec[0] : 0, r1 = n_groups ? group_rec[n_groups] : 0;
-    for (uint64_t i = r0; i < r1; ++i)
-      if (!record_ok(records, rec_off, i)) {
-        g->last_error = "fgb_grouper_add_groups: record " + std::to_string(i) + " is malformed";
-        return FGB_ERR_LAYOUT;
-      }
-    std::vector<GroupPrep> prep(n_groups);
-    std::vector<std::string> err(n_groups);
-    fgb_umi::parallel_for(n_groups, g->opt.umi.n_threads, [&](uint64_t x) {
-      err[x] = prepare_group(*g, records, rec_off, group_rec[x], group_rec[x + 1], &prep[x]);
-    });
-    for (uint64_t x = 0; x < n_groups; ++x)
-      if (!err[x].empty()) {
-        g->last_error = "fgb_grouper_add_groups: position group " + std::to_string(x) + ": " + err[x];
-        return FGB_ERR_INVALID_ARG;
-      }
+  static const char kWho[] = "fgb_grouper_add_groups";
+  return guarded(&g->last_error, kWho, [&]() -> fgb_status {
+    std::vector<GroupPrep> prep;
+    const fgb_status st = prepare_groups(
+        kWho, records, rec_off, group_rec, n_groups, g->opt.umi.n_threads,
+        [&](uint64_t b, uint64_t e, GroupPrep* gp) { return prepare_group(*g, records, rec_off, b, e, gp); }, &prep,
+        &g->last_error);
+    if (st != FGB_OK) return st;
     g->queue.reserve(g->queue.size() + n_groups);
     for (auto& gp : prep) {
       for (int k = 0; k < 6; ++k) g->stats[FGB_GSTAT_TOTAL + k] += gp.filter[k];
@@ -472,7 +406,7 @@ fgb_status fgb_grouper_add_groups(fgb_grouper* g, const uint8_t* records, const 
       if (gp.dropped || gp.tpls.empty()) continue;   // nothing of it reaches the output
       g->queue.push_back(std::move(gp));
     }
-    g->batch_ready = false;
+    g->batch.ready = false;
     return FGB_OK;
   });
 }
@@ -481,15 +415,9 @@ fgb_status fgb_grouper_pending(fgb_grouper* g, const uint8_t** umis, const uint6
                                const uint64_t** call_off, uint64_t* n_calls, const uint64_t** group_off,
                                uint64_t* n_groups) {
   if (!g || !umis || !umi_off || !n_umis || !call_off || !n_calls || !group_off || !n_groups) return FGB_ERR_INVALID_ARG;
-  return guard(g, "fgb_grouper_pending", [&]() -> fgb_status {
-    build_batch(g);
-    *umis = g->b_umis.data();
-    *umi_off = g->b_umi_off.data();
-    *n_umis = g->b_umi_off.size() - 1;
-    *call_off = g->b_call_off.data();
-    *n_calls = g->b_call_off.size() - 1;
-    *group_off = g->b_group_off.data();
-    *n_groups = g->b_group_off.size() - 1;
+  return guarded(&g->last_error, "fgb_grouper_pending", [&]() -> fgb_status {
+    g->batch.build(g->queue);
+    g->batch.pending(umis, umi_off, n_umis, call_off, n_calls, group_off, n_groups);
     return FGB_OK;
   });
 }
@@ -497,22 +425,14 @@ fgb_status fgb_grouper_pending(fgb_grouper* g, const uint8_t** umis, const uint6
 fgb_status fgb_grouper_flush(fgb_grouper* g, const uint8_t** out, uint64_t* out_len, uint64_t* n_records) {
   if (!g || !out || !out_len || !n_records) return FGB_ERR_INVALID_ARG;
   if (!g->h) { g->last_error = "fgb_grouper_flush: a planning-only grouper has no device"; return FGB_ERR_NO_DEVICE; }
-  return guard(g, "fgb_grouper_flush", [&]() -> fgb_status {
-    build_batch(g);
-    const uint64_t n = g->b_umi_off.size() - 1, nc = g->b_call_off.size() - 1, ng = g->b_group_off.size() - 1;
+  return guarded(&g->last_error, "fgb_grouper_flush", [&]() -> fgb_status {
+    g->batch.build(g->queue);
+    const uint64_t n = g->batch.n_umis(), ng = g->batch.n_groups();
     std::vector<uint64_t> ids(n + 1), counts(ng + 1);
     std::vector<uint8_t> kinds(n + 1);
-    static const uint8_t kNoBytes = 0;   // every UMI empty (no_umi): the ABI still wants a pointer
-    const uint8_t* umis = g->b_umis.empty() ? &kNoBytes : g->b_umis.data();
-    const fgb_status st = fgb_umi_assign(g->h, &g->umi, umis, g->b_umi_off.data(), n,
-                                         g->b_call_off.data(), nc, g->b_group_off.data(), ng, ids.data(),
-                                         kinds.data(), counts.data());
-    if (st != FGB_OK) {
-      std::string e(fgb_last_error(g->h, nullptr, 0), '\0');
-      fgb_last_error(g->h, &e[0], e.size() + 1);
-      g->last_error = "fgb_grouper_flush: " + e;
-      return st;
-    }
+    const fgb_status st = g->batch.assign(g->h, g->umi, "fgb_grouper_flush", ids.data(), kinds.data(), counts.data(),
+                                          &g->last_error);
+    if (st != FGB_OK) return st;
     fgb_umi_last_timing(g->h, g->timing);
     const auto t0 = std::chrono::steady_clock::now();
     const fgb_status fs = finish_flush(g, ids.data(), kinds.data(), counts.data(), out, out_len, n_records);
@@ -531,9 +451,9 @@ fgb_status fgb_grouper_flush_with_ids(fgb_grouper* g, const uint64_t* ids, const
                                       const uint64_t* group_mi_count, const uint8_t** out, uint64_t* out_len,
                                       uint64_t* n_records) {
   if (!g || !out || !out_len || !n_records) return FGB_ERR_INVALID_ARG;
-  return guard(g, "fgb_grouper_flush_with_ids", [&]() -> fgb_status {
-    build_batch(g);
-    const uint64_t n = g->b_umi_off.size() - 1, ng = g->b_group_off.size() - 1;
+  return guarded(&g->last_error, "fgb_grouper_flush_with_ids", [&]() -> fgb_status {
+    g->batch.build(g->queue);
+    const uint64_t n = g->batch.n_umis(), ng = g->batch.n_groups();
     if ((n && (!ids || !kinds)) || (ng && !group_mi_count)) return FGB_ERR_INVALID_ARG;
     for (uint64_t u = 0; u < n; ++u)
       if (kinds[u] > FGB_MOL_B) { g->last_error = "fgb_grouper_flush_with_ids: unknown kind"; return FGB_ERR_INVALID_ARG; }
@@ -550,13 +470,7 @@ fgb_status fgb_grouper_stats(const fgb_grouper* g, uint64_t stats[FGB_GROUP_NSTA
 fgb_status fgb_grouper_histogram(const fgb_grouper* g, int which, uint64_t* sizes, uint64_t* counts, uint64_t cap,
                                  uint64_t* n) {
   if (!g || !n || (which != FGB_GROUP_HIST_FAMILY && which != FGB_GROUP_HIST_POSITION)) return FGB_ERR_INVALID_ARG;
-  const auto& h = which == FGB_GROUP_HIST_FAMILY ? g->family_sizes : g->group_sizes;
-  *n = h.size();
-  if (cap < h.size()) return FGB_OK;
-  if (h.size() && (!sizes || !counts)) return FGB_ERR_INVALID_ARG;
-  uint64_t i = 0;
-  for (const auto& [s, c] : h) { sizes[i] = s; counts[i] = c; ++i; }
-  return FGB_OK;
+  return copy_histogram(which == FGB_GROUP_HIST_FAMILY ? g->family_sizes : g->group_sizes, sizes, counts, cap, n);
 }
 
 }  // extern "C"

@@ -1,9 +1,12 @@
 // Record rules `fgumi group` and `fgumi dedup` share: record checks, the aux walk of their filters (MQ and the UMI in
 // one pass), the unclipped 5' end, the pair-orientation split with each template's UMI, and update_string_tag on
-// output.  Used by group_host.cpp and dedup_host.cpp; the citations are to fgumi 0.2.0 as there.
+// output; then the queue both keep around fgb_umi_assign.  Used by group_host.cpp and dedup_host.cpp; the citations are
+// to fgumi 0.2.0 as there.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
+#include <map>
 #include <numeric>
 #include <string>
 #include <string_view>
@@ -11,6 +14,7 @@
 
 #include "../../../include/fgumi_b200.h"
 #include "bam.h"
+#include "umi_host.h"
 
 namespace fgb {
 namespace grp {
@@ -283,6 +287,150 @@ inline void mi_string(uint8_t kind, uint64_t id, uint64_t base, std::string* mi)
 // MoleculeId::to_vec_index + 1 (lib.rs:112-119), 0 for None, so that None sorts first
 inline uint64_t vec_index(uint8_t kind, uint64_t id) {
   return kind == FGB_MOL_NONE ? 0 : kind == FGB_MOL_SINGLE ? id + 1 : 2 * id + (kind == FGB_MOL_B) + 1;
+}
+
+// ---- the queue of the grouper and the deduper around fgb_umi_assign ----------------------------------------------
+
+// The device handle of a grouper or deduper (none for FGB_DEVICE_NONE).  The assignment reads none of the consensus
+// parameters; fgb_create only wants them valid.
+inline fgb_status open_handle(int device, fgb_handle** h) {
+  if (device == FGB_DEVICE_NONE) return FGB_OK;
+  fgb_params p{};
+  p.error_rate_pre_umi = 45;
+  p.error_rate_post_umi = 40;
+  p.min_consensus_base_quality = 40;
+  p.min_reads = 1;
+  return fgb_create(device, &p, h);
+}
+
+// fgb_*_add_groups up to the queue: the group table and every record it covers checked, then prepare(b, e, &(*prep)[x])
+// for the records [b, e) of each position group x on n_threads.  A failure leaves "<who>: ..." in *err.
+template <class G, class Prepare>
+fgb_status prepare_groups(const char* who, const uint8_t* records, const uint64_t* rec_off, const uint64_t* group_rec,
+                          uint64_t n_groups, uint32_t n_threads, Prepare&& prepare, std::vector<G>* prep,
+                          std::string* err) {
+  for (uint64_t x = 0; x < n_groups; ++x)
+    if (group_rec[x + 1] < group_rec[x]) { *err = std::string(who) + ": group_rec descends"; return FGB_ERR_LAYOUT; }
+  const uint64_t r0 = n_groups ? group_rec[0] : 0, r1 = n_groups ? group_rec[n_groups] : 0;
+  for (uint64_t i = r0; i < r1; ++i)
+    if (!record_ok(records, rec_off, i)) {
+      *err = std::string(who) + ": record " + std::to_string(i) + " is malformed";
+      return FGB_ERR_LAYOUT;
+    }
+  prep->resize(n_groups);
+  std::vector<std::string> why(n_groups);
+  fgb_umi::parallel_for(n_groups, n_threads, [&](uint64_t x) {
+    why[x] = prepare(group_rec[x], group_rec[x + 1], &(*prep)[x]);
+  });
+  for (uint64_t x = 0; x < n_groups; ++x)
+    if (!why[x].empty()) {
+      *err = std::string(who) + ": position group " + std::to_string(x) + ": " + why[x];
+      return FGB_ERR_INVALID_ARG;
+    }
+  return FGB_OK;
+}
+
+// The UMI batch of a queue of position groups as fgb_umi_assign takes it: every group's calls and UMIs (its
+// Calls c) back to back, group b's first UMI at call_off[group_off[b]].  Built on demand; ready = false whenever
+// the queue changes.
+struct UmiBatch {
+  bool ready = false;
+  std::vector<uint8_t> umis;
+  std::vector<uint64_t> umi_off, call_off, group_off;
+
+  template <class G>
+  void build(const std::vector<G>& queue) {
+    if (ready) return;
+    umis.clear(); umi_off.assign(1, 0); call_off.assign(1, 0); group_off.assign(1, 0);
+    for (const G& gp : queue) {
+      const uint64_t base = umis.size();
+      umis.insert(umis.end(), gp.c.umis.begin(), gp.c.umis.end());
+      for (uint64_t e : gp.c.umi_end) umi_off.push_back(base + e);
+      const uint64_t ub = call_off.back();
+      for (uint32_t e : gp.c.call_end) call_off.push_back(ub + e);
+      group_off.push_back(call_off.size() - 1);
+    }
+    ready = true;
+  }
+  uint64_t n_umis() const { return umi_off.size() - 1; }
+  uint64_t n_groups() const { return group_off.size() - 1; }
+
+  // fgb_*_pending
+  void pending(const uint8_t** u, const uint64_t** uo, uint64_t* nu, const uint64_t** co, uint64_t* nc,
+               const uint64_t** go, uint64_t* ng) const {
+    *u = umis.data();
+    *uo = umi_off.data();
+    *nu = n_umis();
+    *co = call_off.data();
+    *nc = call_off.size() - 1;
+    *go = group_off.data();
+    *ng = n_groups();
+  }
+
+  // fgb_umi_assign on the batch; a failure leaves "<who>: <the handle's error>" in *err
+  fgb_status assign(fgb_handle* h, const fgb_umi_options& umi, const char* who, uint64_t* ids, uint8_t* kinds,
+                    uint64_t* counts, std::string* err) const {
+    const uint8_t no_bytes = 0;   // every UMI empty (no_umi): the ABI still wants a pointer
+    const fgb_status st = fgb_umi_assign(h, &umi, umis.empty() ? &no_bytes : umis.data(), umi_off.data(), n_umis(),
+                                         call_off.data(), call_off.size() - 1, group_off.data(), n_groups(), ids,
+                                         kinds, counts);
+    if (st != FGB_OK) {
+      std::string e(fgb_last_error(h, nullptr, 0), '\0');
+      fgb_last_error(h, &e[0], e.size() + 1);
+      *err = std::string(who) + ": " + e;
+    }
+    return st;
+  }
+};
+
+// The MI base of each of a flush's ng groups: the counter *next advances by max(id) + 1 = mi_count[b] per group
+// (group.rs:1569-1575, dedup.rs:791-797, 1123-1133).  False, with *next unchanged, when it would overflow.
+inline bool mi_bases(const uint64_t* mi_count, uint64_t ng, uint64_t* next, std::vector<uint64_t>* base) {
+  base->resize(ng);
+  uint64_t at = *next;
+  for (uint64_t b = 0; b < ng; ++b) {
+    (*base)[b] = at;
+    if (at + mi_count[b] < at) return false;
+    at += mi_count[b];
+  }
+  *next = at;
+  return true;
+}
+
+// The groups' output bytes back to back in *out (copied on n_threads), so that the stream is in queue order for any
+// thread count; returns the number of records.
+template <class O>
+uint64_t concat_outputs(const std::vector<O>& outs, uint32_t n_threads, std::vector<uint8_t>* out) {
+  const uint64_t ng = outs.size();
+  std::vector<uint64_t> at(ng + 1, 0);
+  uint64_t recs = 0;
+  for (uint64_t b = 0; b < ng; ++b) { at[b + 1] = at[b] + outs[b].bytes.size(); recs += outs[b].n_records; }
+  out->resize(at[ng]);
+  fgb_umi::parallel_for(ng, n_threads, [&](uint64_t b) {
+    if (!outs[b].bytes.empty()) std::memcpy(out->data() + at[b], outs[b].bytes.data(), outs[b].bytes.size());
+  });
+  return recs;
+}
+
+// fgb_*_histogram: *n entries; sizes / counts filled when cap holds them all
+inline fgb_status copy_histogram(const std::map<uint64_t, uint64_t>& h, uint64_t* sizes, uint64_t* counts,
+                                 uint64_t cap, uint64_t* n) {
+  *n = h.size();
+  if (cap < h.size()) return FGB_OK;
+  if (h.size() && (!sizes || !counts)) return FGB_ERR_INVALID_ARG;
+  uint64_t i = 0;
+  for (const auto& [s, c] : h) { sizes[i] = s; counts[i] = c; ++i; }
+  return FGB_OK;
+}
+
+// fgb_*_last_error: the message's length; as much of it as fits in buf, NUL-terminated
+inline size_t copy_error(const std::string& e, char* buf, size_t buf_len) {
+  if (buf && buf_len) {
+    const size_t n = std::min(buf_len - 1, e.size());
+    std::memcpy(buf, e.data(), n);
+    buf[n] = 0;
+  }
+  return e.size();
 }
 
 // Position grouping of fgb_host_group_by_position and, with include_secondary_supplementary, of

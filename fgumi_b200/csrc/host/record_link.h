@@ -91,15 +91,16 @@ inline fgb_status fail(std::string* last_error, const char* who, cudaError_t e, 
   return e == cudaErrorMemoryAllocation ? FGB_ERR_NOMEM : FGB_ERR_CUDA;
 }
 
-// f() with an escaping exception turned into last_error and FGB_ERR_NOMEM.
+// f() with an escaping exception turned into *last_error and FGB_ERR_NOMEM: no exception crosses the ABI or leaves a
+// std::thread.
 template <class F>
-fgb_status guarded(const HandleInfo& hi, const char* who, F&& f) {
+fgb_status guarded(std::string* last_error, const char* who, F&& f) {
   try {
     return f();
   } catch (const std::bad_alloc&) {
-    *hi.last_error = std::string(who) + ": out of host memory";
+    *last_error = std::string(who) + ": out of host memory";
   } catch (const std::exception& x) {
-    *hi.last_error = std::string(who) + ": " + x.what();
+    *last_error = std::string(who) + ": " + x.what();
   }
   return FGB_ERR_NOMEM;
 }

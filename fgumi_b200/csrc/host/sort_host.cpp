@@ -389,7 +389,7 @@ fgb_status fgb_sort_records(fgb_handle* h, const fgb_sort_options* opt, const ch
   if (hi.busy) { *hi.last_error = "fgb_sort_records: a submit has not been waited on"; return FGB_ERR_BUSY; }
   *out_len = need;
   if (!n_records) return FGB_OK;
-  return link::guarded(hi, "fgb_sort_records", [&] {
+  return link::guarded(hi.last_error, "fgb_sort_records", [&] {
     return sort_impl(hi, *opt, std::string_view(header_text ? header_text : "", header_len), records, rec_off,
                      n_records, out);
   });

@@ -369,7 +369,7 @@ fgb_status fgb_zipper_records(fgb_handle* h, const fgb_zipper_options* opt, cons
   if (hi.busy) { *hi.last_error = "fgb_zipper_records: a submit has not been waited on"; return FGB_ERR_BUSY; }
   const Stream us{unmapped, u_off, n_unmapped, 0, false}, ms{mapped, m_off, n_mapped, n_unmapped, true};
   Fail fl;
-  const fgb_status st = link::guarded(hi, "fgb_zipper_records", [&]() -> fgb_status {
+  const fgb_status st = link::guarded(hi.last_error, "fgb_zipper_records", [&]() -> fgb_status {
     hi.kept->clear();
     return zipper_impl(hi, *opt, us, ms, last_call != 0, mapped_consumed, stats, &fl);
   });

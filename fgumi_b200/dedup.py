@@ -16,6 +16,7 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 
 from . import lib as _l
+from .group import _AssignQueue, _group_by_position
 from .umi import options as _umi_options
 
 METRIC_NAMES = ("total_templates", "unique_templates", "duplicate_templates", "duplicate_rate", "total_reads",
@@ -26,24 +27,7 @@ def group_by_position(bodies: np.ndarray, rec_off: np.ndarray, header_text: byte
                       cell_tag: Optional[bytes] = b"CB") -> Tuple[np.ndarray, np.ndarray]:
     """(keep mask, all ones; group table over the records).  A paired mapped primary record with a mapped mate and no
     MC tag raises ValueError naming the record."""
-    lib = _l.load()
-    n = len(rec_off) - 1
-    keep = np.zeros(max(n, 1), np.uint8)
-    gb = np.zeros(n + 2, np.uint64)
-    ng, bad = C.c_uint64(), C.c_uint64()
-    bodies = np.ascontiguousarray(bodies, np.uint8)
-    rec_off = np.ascontiguousarray(rec_off, np.uint64)
-    st = lib.fgb_host_dedup_group_by_position(bodies.ctypes.data, rec_off.ctypes.data, n, header_text,
-                                              len(header_text), cell_tag, keep.ctypes.data, gb.ctypes.data,
-                                              C.byref(ng), C.byref(bad))
-    if st == _l.FGB_ERR_INVALID_ARG and bad.value < n:
-        i = bad.value
-        rec = bodies[int(rec_off[i]):int(rec_off[i + 1])].tobytes()
-        raise ValueError(f"record {i} ({rec[32:32 + rec[8] - 1].decode(errors='replace')}): paired-end reads need "
-                         "MC tags for position grouping")
-    if st != _l.FGB_OK:
-        raise _l.FgbError(st, "fgb_host_dedup_group_by_position")
-    return keep[:n], gb[:ng.value + 1]
+    return _group_by_position("fgb_host_dedup_group_by_position", bodies, rec_off, header_text, cell_tag)
 
 
 def dedup_metrics(stats: Dict[str, int]) -> dict:
@@ -70,15 +54,17 @@ def record_quality_scores(engine, bodies: np.ndarray, rec_off: np.ndarray) -> np
     return out[:n]
 
 
-class Deduper:
+class Deduper(_AssignQueue):
     """fgb_deduper_* on one GPU; device=None gives a planning-only deduper (pending / flush_with_ids)."""
+    _prefix, _stat_names, _n_stats = "fgb_deduper", _l.DEDUP_STAT_NAMES, _l.FGB_DEDUP_NSTATS
+    _timing_names = ("prepare_ms", "device_phase_ms", "kernels_ms", "resolve_ms", "score_phase_ms", "score_kernel_ms",
+                    "emit_ms")
 
     def __init__(self, device: Optional[int] = 0, strategy: str = "adjacency", edits: int = 1,
                  min_umi_length: Optional[int] = None, min_map_q: int = 0, include_non_pf: bool = False,
                  no_umi: bool = False, remove_duplicates: bool = False, umi_tag: bytes = b"RX",
                  assign_tag: bytes = b"MI", first_mi: int = 0, n_threads: int = 1):
         self._lib = _l.load()
-        self._h = None
         u = _umi_options(strategy, 0 if strategy == "identity" else edits, "mapped", min_umi_length, n_threads)
         self.opt = _l.FgbDedupOptions(u, min_map_q, int(include_non_pf), int(no_umi), int(remove_duplicates),
                                       umi_tag, assign_tag, first_mi)
@@ -89,53 +75,6 @@ class Deduper:
             raise _l.FgbError(st, "fgb_deduper_create")
         self._h = h
 
-    def close(self):
-        if self._h:
-            self._lib.fgb_deduper_destroy(self._h)
-            self._h = None
-
-    def __del__(self):  # pragma: no cover
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _check(self, st: int, where: str):
-        if st != _l.FGB_OK:
-            buf = C.create_string_buffer(1024)
-            self._lib.fgb_deduper_last_error(self._h, buf, len(buf))
-            raise _l.FgbError(st, where, buf.value.decode(errors="replace"))
-
-    def add_groups(self, bodies: np.ndarray, rec_off: np.ndarray, groups: np.ndarray):
-        bodies = np.ascontiguousarray(bodies, np.uint8)
-        rec_off = np.ascontiguousarray(rec_off, np.uint64)
-        groups = np.ascontiguousarray(groups, np.uint64)
-        self._check(self._lib.fgb_deduper_add_groups(self._h, bodies.ctypes.data, rec_off.ctypes.data,
-                                                     groups.ctypes.data, len(groups) - 1), "fgb_deduper_add_groups")
-
-    def pending(self):
-        """The queued UMI batch as fgb_umi_assign would receive it: groups -> calls -> UMIs (bytes)."""
-        um, uo, co, go = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
-        nu, nc, ng = C.c_uint64(), C.c_uint64(), C.c_uint64()
-        self._check(self._lib.fgb_deduper_pending(self._h, C.byref(um), C.byref(uo), C.byref(nu), C.byref(co),
-                                                  C.byref(nc), C.byref(go), C.byref(ng)), "fgb_deduper_pending")
-
-        def arr(p, n):
-            return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint64)), (n,)).copy()
-        uoff, coff, goff = arr(uo, nu.value + 1), arr(co, nc.value + 1), arr(go, ng.value + 1)
-        blob = C.string_at(um.value, int(uoff[-1])) if uoff[-1] else b""
-        umis = [blob[int(uoff[i]):int(uoff[i + 1])] for i in range(nu.value)]
-        calls = [umis[int(coff[c]):int(coff[c + 1])] for c in range(nc.value)]
-        return [calls[int(goff[g]):int(goff[g + 1])] for g in range(ng.value)]
-
-    def _take(self, data, n) -> bytes:
-        return C.string_at(data.value, n.value) if n.value else b""
-
-    def flush(self) -> bytes:
-        data, n, cnt = C.c_void_p(), C.c_uint64(), C.c_uint64()
-        self._check(self._lib.fgb_deduper_flush(self._h, C.byref(data), C.byref(n), C.byref(cnt)), "fgb_deduper_flush")
-        return self._take(data, n)
-
     def flush_with_ids(self, kinds, ids, group_mi_count, scores) -> bytes:
         """Completes the flush from an assignment and template scores computed elsewhere, each indexed like the
         flattened pending() batch."""
@@ -144,33 +83,23 @@ class Deduper:
         kinds, ids, cnt_in, sc = (flat(kinds, np.uint8), flat(ids, np.uint64), flat(group_mi_count, np.uint64),
                                   flat(scores, np.uint32))
         data, n, cnt = C.c_void_p(), C.c_uint64(), C.c_uint64()
-        self._check(self._lib.fgb_deduper_flush_with_ids(self._h, ids.ctypes.data, kinds.ctypes.data,
-                                                         cnt_in.ctypes.data, sc.ctypes.data, C.byref(data),
-                                                         C.byref(n), C.byref(cnt)), "fgb_deduper_flush_with_ids")
+        self._call("flush_with_ids", ids.ctypes.data, kinds.ctypes.data, cnt_in.ctypes.data, sc.ctypes.data,
+                   C.byref(data), C.byref(n), C.byref(cnt))
         return self._take(data, n)
-
-    def stats(self) -> Dict[str, int]:
-        s = (C.c_uint64 * _l.FGB_DEDUP_NSTATS)()
-        self._check(self._lib.fgb_deduper_stats(self._h, s), "fgb_deduper_stats")
-        return dict(zip(_l.DEDUP_STAT_NAMES, list(s)))
 
     def histogram(self) -> Dict[int, int]:
         """Family sizes over every flush so far (unassigned templates skipped)."""
         n = C.c_uint64()
-        self._check(self._lib.fgb_deduper_histogram(self._h, None, None, 0, C.byref(n)), "fgb_deduper_histogram")
+        self._call("histogram", None, None, 0, C.byref(n))
         sizes = np.zeros(max(n.value, 1), np.uint64)
         counts = np.zeros(max(n.value, 1), np.uint64)
-        self._check(self._lib.fgb_deduper_histogram(self._h, sizes.ctypes.data, counts.ctypes.data, n.value,
-                                                    C.byref(n)), "fgb_deduper_histogram")
+        self._call("histogram", sizes.ctypes.data, counts.ctypes.data, n.value, C.byref(n))
         return {int(s): int(c) for s, c in zip(sizes[:n.value], counts[:n.value])}
 
     def last_timing(self) -> Dict[str, float]:
         """ms of the last flush: the assignment's host key tables, device phase, edge kernels (CUDA events) and host
         rules; the score phase as the host saw it and its kernel (CUDA events); then selection, flags and emit."""
-        ms = (C.c_double * 7)()
-        self._check(self._lib.fgb_deduper_last_timing(self._h, ms), "fgb_deduper_last_timing")
-        return dict(zip(("prepare_ms", "device_phase_ms", "kernels_ms", "resolve_ms", "score_phase_ms",
-                         "score_kernel_ms", "emit_ms"), list(ms)))
+        return super().last_timing()
 
     def metrics(self) -> dict:
         return dedup_metrics(self.stats())
